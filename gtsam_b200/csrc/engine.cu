@@ -278,28 +278,48 @@ static int enqueue_solve(b200_problem* p, bool damped, int diagonal, double min_
                                                            p->d_scalars, p->leaf_lb_cap, 0));
       ctx->launches++;
     }
-    // BAL points: per-point factorisation (8 lanes per point) ...
-    for (int kd = 1; kd <= 2; kd++) {
+    // BAL points.  schur_mma (default): one CTA per run of points with the same cameras factors the run's points and adds
+    // their Schur complement into the parent on the FP64 tensor path, in one kernel
+    for (int kd = 1; kd <= 2 && p->schur_mma; kd++) {
+      const int nr = p->leaf_run_end[kd] - p->leaf_run_begin[kd];
+      if (nr <= 0) continue;
+      const int* runs = p->d_fused_run_ptr + p->leaf_run_begin[kd];
+      const int dc = kd == 1 ? 6 : 9, maxw = p->leaf_max_w[kd], nt8 = (maxw + 7) / 8;
+      const int mmax = std::max(1, (maxw - 1) / dc), sa = (dc < 8 ? 8 : 16) * kSmPA + kSmPadA;
+      const size_t jb = p->jac_f32 ? sizeof(float) : sizeof(double);
+      // leaf_point_fused_mma_kernel's layout: per warp [R S' d']^T, then per warp [A_c b]^T (two buffers) and A_p (two
+      // buffers); the four warps' Schur sums (8 nt8)^2 reuse it at the end
+      const size_t sm = std::max((size_t)4 * (3 + 8 * nt8) * kSmKS * sizeof(double) + (size_t)4 * (2 * mmax * sa + 2 * 6 * 32) * jb,
+                                 (size_t)64 * nt8 * nt8 * sizeof(double));
+      bool done = false;
+#define B200_LAUNCH_FUSED(DC_, T_)                                                                                                    \
+      if (!done && dc == DC_ && nt8 <= T_) {                                                                                          \
+        DISPATCH_JT(p, launch_k(leaf_point_fused_mma_kernel<DC_, T_, JT>, dim3(nr), dim3(128), sm, st, t, gt, (const int*)p->d_fused_list, runs, \
+                 (const double*)p->d_lambda, hd, min_diag, max_diag, p->d_scalars, (const int2*)p->d_pt_tab, (const int64_t*)p->d_pt_off)); \
+        done = true;                                                                                                                  \
+      }
+      B200_LAUNCH_FUSED(6, 4) B200_LAUNCH_FUSED(6, 5) B200_LAUNCH_FUSED(6, 7)
+      B200_LAUNCH_FUSED(9, 4) B200_LAUNCH_FUSED(9, 5) B200_LAUNCH_FUSED(9, 7) B200_LAUNCH_FUSED(9, 10)
+#undef B200_LAUNCH_FUSED
+      if (!done) { set_error("leaf_point_fused_mma_kernel: separator wider than the compiled tile counts"); return B200_CUDA_ERROR; }
+      ctx->launches++;
+    }
+    // schur_mma = 0: per-point factorisation (8 lanes per point) ...
+    for (int kd = 1; kd <= 2 && !p->schur_mma; kd++) {
       if (p->leaf_run_end[kd] <= p->leaf_run_begin[kd]) continue;
       const int i0 = p->leaf_pos_begin[kd], i1 = p->leaf_pos_end[kd];
       const int nb = (int)(((int64_t)(i1 - i0) * 8 + 127) / 128);
-      const int ncap = 3 * (3 + p->leaf_max_w[kd]);     // staged variant: doubles per point in shared memory
 #define B200_LAUNCH_POINT(DC_)                                                                                                        \
-      if (p->factor_staged)                                                                                                           \
-      DISPATCH_JT(p, launch_k(leaf_point_factor_kernel<DC_, JT, true>, dim3(nb), dim3(128), (size_t)16 * ncap * sizeof(double), st, t, gt, (const int*)p->d_fused_list, i0, i1, \
+      DISPATCH_JT(p, launch_k(leaf_point_factor_kernel<DC_, JT>, dim3(nb), dim3(128), 0, st, t, gt, (const int*)p->d_fused_list, i0, i1, \
                (const int*)p->d_fused_fac_ptr, (const int2*)p->d_fused_fac, (const double*)p->d_lambda, hd, min_diag, max_diag,        \
-               p->d_scalars, ncap, (const int2*)p->d_pt_tab, (const int64_t*)p->d_pt_off));                                           \
-      else                                                                                                                            \
-      DISPATCH_JT(p, launch_k(leaf_point_factor_kernel<DC_, JT, false>, dim3(nb), dim3(128), 0, st, t, gt, (const int*)p->d_fused_list, i0, i1, \
-               (const int*)p->d_fused_fac_ptr, (const int2*)p->d_fused_fac, (const double*)p->d_lambda, hd, min_diag, max_diag,        \
-               p->d_scalars, ncap, (const int2*)p->d_pt_tab, (const int64_t*)p->d_pt_off));
+               p->d_scalars, (const int2*)p->d_pt_tab, (const int64_t*)p->d_pt_off));
       if (kd == 1) { B200_LAUNCH_POINT(6) } else { B200_LAUNCH_POINT(9) }
 #undef B200_LAUNCH_POINT
       ctx->launches++;
     }
   }
-  if (p->n_fused) {
-    // ... then one CTA per run of points with the same cameras for the Schur complement
+  if (p->n_fused && !p->schur_mma) {
+    // ... then one CTA per run of points with the same cameras for the Schur complement (3x3 FMA tiles)
     PhaseScope ps(p, PH_LEAF_SCHUR);
     GroupTable gt;
     for (size_t gi = 0; gi < p->groups.size(); gi++) gt.g[gi] = view(p->groups[gi]);
@@ -307,26 +327,6 @@ static int enqueue_solve(b200_problem* p, bool damped, int diagonal, double min_
       const int nr = p->leaf_run_end[kd] - p->leaf_run_begin[kd];
       if (nr <= 0) continue;
       const int* runs = p->d_fused_run_ptr + p->leaf_run_begin[kd];
-      if (p->schur_mma) {
-        // FP64 tensor path: 8x8 DMMA tiles over (s+1)^2 / 2 and per camera; every warp stages and multiplies its own points
-        const int dc = kd == 1 ? 6 : 9, maxw = p->leaf_max_w[kd], nt8 = (maxw + 7) / 8;
-        const int mmax = std::max(1, (maxw - 1) / dc), cp = dc < 8 ? 8 : 16;
-        const size_t jb = p->jac_f32 ? sizeof(float) : sizeof(double);
-        const size_t sm = (size_t)4 * 2 * 8 * nt8 * kSmKS * sizeof(double) + (size_t)4 * 2 * mmax * cp * kSmPA * jb;
-        bool done = false;
-#define B200_LAUNCH_SCHUR_MMA(DC_, T_)                                                                                                \
-        if (!done && dc == DC_ && nt8 <= T_) {                                                                                        \
-          DISPATCH_JT(p, launch_k(leaf_point_schur_mma_kernel<DC_, T_, JT>, dim3(nr), dim3(128), sm, st, t, gt, (const int*)p->d_fused_list, runs, \
-                   (const int2*)p->d_pt_tab, (const int64_t*)p->d_pt_off));                                                          \
-          done = true;                                                                                                                \
-        }
-        B200_LAUNCH_SCHUR_MMA(6, 4) B200_LAUNCH_SCHUR_MMA(6, 5) B200_LAUNCH_SCHUR_MMA(6, 7)
-        B200_LAUNCH_SCHUR_MMA(9, 4) B200_LAUNCH_SCHUR_MMA(9, 5) B200_LAUNCH_SCHUR_MMA(9, 7) B200_LAUNCH_SCHUR_MMA(9, 10)
-#undef B200_LAUNCH_SCHUR_MMA
-        if (!done) { set_error("leaf_point_schur_mma_kernel: separator wider than the compiled tile counts"); return B200_CUDA_ERROR; }
-        ctx->launches++;
-        continue;
-      }
       // CTA shape from the widest separator of the kind: 3x3 tiles over (s+1)^2 / 2
       const int ntd = (p->leaf_max_w[kd] + 2) / 3, ntiles = ntd * (ntd + 1) / 2;
       const int thr = ntiles <= 96 ? 96 : 128, tpt = (ntiles + thr - 1) / thr;
@@ -1261,14 +1261,13 @@ static int create_problem(b200_ctx* ctx, const b200_problem_desc* d, const b200_
   p->fuse_ea = getenv("B200_NO_FUSE_EA") == nullptr;
   p->schur_pb = (getenv("B200_SCHUR_PB") && atoi(getenv("B200_SCHUR_PB")) == 6) ? 6 : 4;
   p->schur_mma = !(getenv("B200_SCHUR_MMA") && atoi(getenv("B200_SCHUR_MMA")) == 0);
-  p->factor_staged = !(getenv("B200_FACTOR_STAGED") && atoi(getenv("B200_FACTOR_STAGED")) == 0);
   if (getenv("B200_LIN_VARIANT")) p->lin_variant = atoi(getenv("B200_LIN_VARIANT"));
 #ifndef B200_EMULATE
   {   // the widest instantiations stage more than the 48 KB a kernel gets by default
     const int optin = 200 * 1024;
 #define B200_SM_ATTR(DC_, T_)                                                                                                          \
-    B200_CUDA(cudaFuncSetAttribute(leaf_point_schur_mma_kernel<DC_, T_, double>, cudaFuncAttributeMaxDynamicSharedMemorySize, optin)); \
-    B200_CUDA(cudaFuncSetAttribute(leaf_point_schur_mma_kernel<DC_, T_, float>, cudaFuncAttributeMaxDynamicSharedMemorySize, optin));
+    B200_CUDA(cudaFuncSetAttribute(leaf_point_fused_mma_kernel<DC_, T_, double>, cudaFuncAttributeMaxDynamicSharedMemorySize, optin)); \
+    B200_CUDA(cudaFuncSetAttribute(leaf_point_fused_mma_kernel<DC_, T_, float>, cudaFuncAttributeMaxDynamicSharedMemorySize, optin));
     B200_SM_ATTR(6, 4) B200_SM_ATTR(6, 5) B200_SM_ATTR(6, 7) B200_SM_ATTR(9, 4) B200_SM_ATTR(9, 5) B200_SM_ATTR(9, 7) B200_SM_ATTR(9, 10)
 #undef B200_SM_ATTR
   }
@@ -2026,7 +2025,7 @@ int b200_set_tuning(b200_problem* p, const char* key, int64_t value) {
   const std::string k(key);
   if (k == "schur_mma") p->schur_mma = value != 0;
   else if (k == "lin_variant") p->lin_variant = (int)value;
-  else if (k == "factor_staged") p->factor_staged = value != 0;
+  else if (k == "factor_staged") {}   // accepted, no effect: the split path stores the point conditionals directly
   else if (k == "schur_pb") p->schur_pb = value == 6 ? 6 : 4;
   else if (k == "df_minb") p->df_minb = value == 3 ? 3 : 2;
   else { set_error("b200_set_tuning: unknown key " + k); return B200_INVALID_ARGUMENT; }

@@ -147,8 +147,7 @@ struct b200_problem {
   int n_fused = 0, n_runs = 0, leaf_lb_cap = 1, leaf_acc_cap = 0;
   int leaf_run_begin[3] = {0, 0, 0}, leaf_run_end[3] = {0, 0, 0};  // run ranges: generic / point DC=6 / point DC=9
   int schur_pb = 4;                                                 // points per staged batch of leaf_point_schur_kernel
-  bool schur_mma = true;                                            // per-run Schur complement on the FP64 tensor path (leaf_point_schur_mma_kernel)
-  bool factor_staged = true;                                        // leaf_point_factor_kernel: conditional staged in shared memory, coalesced stores
+  bool schur_mma = true;                                            // BAL point leaves: factor + per-run Schur complement on the FP64 tensor path in one kernel (leaf_point_fused_mma_kernel)
   int lin_variant = 0;                                              // linearize_kernel variant of the projection groups (b200_set_tuning)
   int leaf_max_w[3] = {1, 1, 1};                                    // widest separator + 1 per kind
   int leaf_pos_begin[3] = {0, 0, 0}, leaf_pos_end[3] = {0, 0, 0};  // the same ranges as positions in d_fused_list

@@ -3,9 +3,11 @@
 //  linearize_kernel      a1-a7   residual + Jacobian + whitening (+ robust reweighting), one thread per
 //                                factor, element-major SoA stores => every store instruction coalesced
 //  error_kernel          a8      0.5*|R r|^2 or rho(|R r|); single launch, last-block reduction in index order
-//  leaf_point_factor_kernel<DC>    a10+a12+a13+a14  BAL point cliques, per-point half: assemble + damp + 3x3 Cholesky, 8 lanes per point
-//  leaf_point_schur_kernel<DC,..>  a12  per-run half: SYRK of the run's Schur complement (3x3 register tiles, cp.async
-//                                staging), one extend-add per run of points with the same cameras
+//  leaf_point_fused_mma_kernel<DC,..>  a10+a12+a13+a14  BAL point cliques, one CTA per run of points with the same
+//                                cameras: per point assemble + damp + 3x3 Cholesky (8 lanes per point), the run's Schur
+//                                complement as FP64 DMMA tiles, one extend-add per run
+//  leaf_point_factor_kernel<DC>, leaf_point_schur_kernel<DC,..>  the same in two kernels (schur_mma = 0): per point,
+//                                then the per-run SYRK in 3x3 register tiles
 //  leaf_fused_kernel     a10+a12+a13+a14  any leaf clique with a small frontal block
 //  assemble_kernel       a12     J^T J / J^T b / b^T b scatter-add into the owning non-leaf front
 //  hdiag_kernel, damp_kernel  a10  hessianDiagonal; lambda*I or lambda*clip(diag H) on the diagonal
@@ -813,16 +815,15 @@ leaf_fused_kernel(TreeView t, GroupTable gt, const int* __restrict__ list, const
 // BAL fast path of the fused leaf elimination: cliques whose single frontal variable is a Point3
 // observed by m <= kPtMaxObs DISTINCT cameras through binary projection factors
 // (GenericProjectionFactor: DC = 6, GeneralSFMFactor<Cal3Bundler>: DC = 9).  Same maths and same
-// outputs as leaf_fused_kernel, split into a per-point and a per-run kernel:
+// outputs as leaf_fused_kernel.  Per point, 8 lanes (one LANE per factor) assemble H_pp / g_p, damp, factor the 3x3
+// block in registers and form S' = R^-T H_pc, d' = R^-T g_p: the compact conditional [R S' d'] (3 x n), PointFactor.
+// Per RUN of points seen by the same cameras, the Schur complement  sum_p ( [A_c b]^T [A_c b] - [S' d']^T [S' d'] )  is a
+// small SYRK (K = 3 per point, N = s + 1), added into the parent with ONE extend-add (FP64 atomics) per run.
 //
-//  leaf_point_factor_kernel  8 lanes per point (one LANE per factor): assemble H_pp / g_p, damp,
-//      3x3 Cholesky in registers, S' = R^-T H_pc, d' = R^-T g_p; writes the compact conditional
-//      [R S' d'] (3 x n).  50k points = 12.5k warps, nothing sequential: latency is hidden by
-//      occupancy instead of being paid per point.
-//  leaf_point_schur_kernel   one CTA per RUN of points seen by the same cameras.  The run's Schur
-//      complement  sum_p ( [A_c b]^T [A_c b] - [S' d']^T [S' d'] )  is a small SYRK (K = 3 per
-//      point, N = s + 1): 3x3 register tiles over the (s+1)^2 upper triangle, operands staged in
-//      shared memory 8 points at a time, ONE extend-add (FP64 atomics) per run into the parent.
+//  leaf_point_fused_mma_kernel (default)  both, one CTA per run; the SYRK as 8x8 DMMA tiles (below).
+//  leaf_point_factor_kernel + leaf_point_schur_kernel (schur_mma = 0)  a per-point kernel (50k points = 12.5k warps,
+//      latency hidden by occupancy), then one CTA per run with 3x3 register tiles over the (s+1)^2 upper triangle and
+//      the operands staged in shared memory 4 or 6 points at a time.
 // ---------------------------------------------------------------------------
 constexpr int kPtMaxObs = 8;
 
@@ -850,15 +851,85 @@ template <int N>
 __device__ __forceinline__ void cp_async_wait() { asm volatile("cp.async.wait_group %0;\n" ::"n"(N)); }
 #endif
 
-// STAGED: the conditional [R S' d'] of the warp's 4 points goes through shared memory and leaves as contiguous 256-byte
-// store instructions.  Direct (STAGED = false): every lane stores its camera's 3 x DC block 8 bytes at a time, 3 DC * 8 bytes
-// apart from its neighbour's — each 32-byte sector is written by four separate instructions, which keeps L2 busier than
-// DRAM.  ncap = doubles reserved per point (3 x the widest n of the kind).
-template <int DC, typename JT = double, bool STAGED = false>
+// The per-point arithmetic of the BAL point leaves.  leaf_point_factor_kernel and leaf_point_fused_mma_kernel both go
+// through it, so the two store bitwise the same conditionals: every product and fused multiply-add is spelled out
+// (fma / mul_rn), since where the compiler would contract a * b + c on its own depends on the surrounding kernel.
+// 8 lanes per point, one factor per lane.
+#ifdef B200_EMULATE
+__device__ __forceinline__ double mul_rn(double a, double b) { return a * b; }
+#else
+__device__ __forceinline__ double mul_rn(double a, double b) { return __dmul_rn(a, b); }
+#endif
+struct PointFactor {
+  double r00, r01, r02, r11, r12, r22, i00, i11, i22;   // R (upper) and the reciprocals of its diagonal
+  double d0, d1, d2;                                    // d' = R^-T g_p
+  bool ok;
+  // this lane's factor's share of [H_pp g_p]: the upper triangle of A_p^T A_p (6) and A_p^T b (3)
+  __device__ __forceinline__ static void lane_terms(const double Ap[2][3], const double b[2], double v[9]) {
+    v[0] = fma(Ap[0][0], Ap[0][0], mul_rn(Ap[1][0], Ap[1][0]));
+    v[1] = fma(Ap[0][0], Ap[0][1], mul_rn(Ap[1][0], Ap[1][1]));
+    v[2] = fma(Ap[0][0], Ap[0][2], mul_rn(Ap[1][0], Ap[1][2]));
+    v[3] = fma(Ap[0][1], Ap[0][1], mul_rn(Ap[1][1], Ap[1][1]));
+    v[4] = fma(Ap[0][1], Ap[0][2], mul_rn(Ap[1][1], Ap[1][2]));
+    v[5] = fma(Ap[0][2], Ap[0][2], mul_rn(Ap[1][2], Ap[1][2]));
+    v[6] = fma(Ap[0][0], b[0], mul_rn(Ap[1][0], b[1]));
+    v[7] = fma(Ap[0][1], b[0], mul_rn(Ap[1][1], b[1]));
+    v[8] = fma(Ap[0][2], b[0], mul_rn(Ap[1][2], b[1]));
+  }
+  // v: the lane's terms; summed over the point's 8 lanes, damped (lambda, times the clipped diagonal of H at the point's
+  // variables di when hd is given), then the 3x3 partial Cholesky in registers (every lane of the point, identical):
+  // gtsam/base/cholesky.cpp:107-158 (rsqrt + multiplies instead of sqrt + divides: same result to ~1 ulp per operation,
+  // a third of the latency)
+  __device__ __forceinline__ void factor(double v[9], double lambda, const double* __restrict__ hd, const int* __restrict__ di,
+                                         double min_diag, double max_diag) {
+#pragma unroll
+    for (int i = 0; i < 9; i++)
+#pragma unroll
+      for (int o = 4; o > 0; o >>= 1) v[i] += __shfl_xor_sync(0xffffffffu, v[i], o);
+    if (lambda > 0) {
+      const double sl = 1.0 / (1.0 / sqrt(lambda)), sl2 = mul_rn(sl, sl);
+      double a2[3] = {1.0, 1.0, 1.0};
+      if (hd) {
+#pragma unroll
+        for (int i = 0; i < 3; i++) { const double sq = sqrt(fmin(fmax(hd[di[i]], min_diag), max_diag)); a2[i] = mul_rn(sq, sq); }
+      }
+      v[0] = fma(sl2, a2[0], v[0]); v[3] = fma(sl2, a2[1], v[3]); v[5] = fma(sl2, a2[2], v[5]);
+    }
+    ok = v[0] > 0.0;
+    i00 = rsqrt(v[0]);
+    r00 = mul_rn(v[0], i00);
+    r01 = mul_rn(v[1], i00); r02 = mul_rn(v[2], i00);
+    const double p11 = fma(-r01, r01, v[3]);
+    ok = ok && p11 > 0.0;
+    i11 = rsqrt(p11);
+    r11 = mul_rn(p11, i11);
+    r12 = mul_rn(fma(-r01, r02, v[4]), i11);
+    const double p22 = fma(-r12, r12, fma(-r02, r02, v[5]));
+    ok = ok && p22 > 0.0;
+    i22 = rsqrt(p22);
+    r22 = mul_rn(p22, i22);
+    if (!(dexp(r11) - dexp(r22) < 12)) ok = false;
+    d0 = mul_rn(v[6], i00);
+    d1 = mul_rn(fma(-r01, d0, v[7]), i11);
+    d2 = mul_rn(fma(-r12, d1, fma(-r02, d0, v[8])), i22);
+  }
+  // one column of S' = R^-T A_p^T A_c, from the column (a0, a1) of this lane's A_c
+  __device__ __forceinline__ void s_col(const double Ap[2][3], double a0, double a1, double& s0, double& s1, double& s2) const {
+    const double w0 = fma(Ap[0][0], a0, mul_rn(Ap[1][0], a1));
+    const double w1 = fma(Ap[0][1], a0, mul_rn(Ap[1][1], a1));
+    const double w2 = fma(Ap[0][2], a0, mul_rn(Ap[1][2], a1));
+    s0 = mul_rn(w0, i00);
+    s1 = mul_rn(fma(-r01, s0, w1), i11);
+    s2 = mul_rn(fma(-r12, s1, fma(-r02, s0, w2)), i22);
+  }
+};
+
+// The split path (schur_mma = 0): every lane stores its camera's 3 x DC block of the conditional directly.
+template <int DC, typename JT = double>
 __global__ void __launch_bounds__(128)
 leaf_point_factor_kernel(TreeView t, GroupTable gt, const int* __restrict__ list, int i_begin, int i_end,
                          const int* __restrict__ fac_ptr, const int2* __restrict__ fac, const double* __restrict__ lambda_ptr,
-                         const double* __restrict__ hdiag, double min_diag, double max_diag, Scalars* sc, int ncap,
+                         const double* __restrict__ hdiag, double min_diag, double max_diag, Scalars* sc,
                          const int2* __restrict__ pt_tab, const int64_t* __restrict__ pt_off) {
   pdl_sync();
   const double lambda = *lambda_ptr;
@@ -876,9 +947,9 @@ leaf_point_factor_kernel(TreeView t, GroupTable gt, const int* __restrict__ list
   for (int o = 4; o > 0; o >>= 1) m += __shfl_xor_sync(0xffffffffu, m, o);
   double Ac[2][DC], Ap[2][3], b[2];
   int tk = 0;
-  double v[10];
+  double v[9];
 #pragma unroll
-  for (int i = 0; i < 10; i++) v[i] = 0.0;
+  for (int i = 0; i < 9; i++) v[i] = 0.0;
   if (rec.x >= 0) {
     const GroupView& g = gt.g[rec.y >> 8];
     const size_t cnt = (size_t)g.count;
@@ -889,88 +960,28 @@ leaf_point_factor_kernel(TreeView t, GroupTable gt, const int* __restrict__ list
 #pragma unroll
     for (int j = 0; j < 3; j++) { Ap[0][j] = J[(size_t)(2 * (DC + j)) * cnt]; Ap[1][j] = J[(size_t)(2 * (DC + j) + 1) * cnt]; }
     b[0] = J[(size_t)(2 * (DC + 3)) * cnt]; b[1] = J[(size_t)(2 * (DC + 3) + 1) * cnt];
-    v[0] = Ap[0][0] * Ap[0][0] + Ap[1][0] * Ap[1][0];
-    v[1] = Ap[0][0] * Ap[0][1] + Ap[1][0] * Ap[1][1];
-    v[2] = Ap[0][0] * Ap[0][2] + Ap[1][0] * Ap[1][2];
-    v[3] = Ap[0][1] * Ap[0][1] + Ap[1][1] * Ap[1][1];
-    v[4] = Ap[0][1] * Ap[0][2] + Ap[1][1] * Ap[1][2];
-    v[5] = Ap[0][2] * Ap[0][2] + Ap[1][2] * Ap[1][2];
-    v[6] = Ap[0][0] * b[0] + Ap[1][0] * b[1];
-    v[7] = Ap[0][1] * b[0] + Ap[1][1] * b[1];
-    v[8] = Ap[0][2] * b[0] + Ap[1][2] * b[1];
+    PointFactor::lane_terms(Ap, b, v);
   }
-#pragma unroll
-  for (int i = 0; i < 9; i++)
-#pragma unroll
-    for (int o = 4; o > 0; o >>= 1) v[i] += __shfl_xor_sync(0xffffffffu, v[i], o);
-  if (lambda > 0) {
-    const double sl = 1.0 / (1.0 / sqrt(lambda));
-    double a2[3] = {1.0, 1.0, 1.0};
-    if (hdiag && live) {
-      const int* di = t.didx + t.didx_ptr[c];
-#pragma unroll
-      for (int i = 0; i < 3; i++) { const double sq = sqrt(fmin(fmax(hdiag[di[i]], min_diag), max_diag)); a2[i] = sq * sq; }
-    }
-    v[0] += (sl * sl) * a2[0]; v[3] += (sl * sl) * a2[1]; v[5] += (sl * sl) * a2[2];
-  }
-  // 3x3 partial Cholesky in registers (every lane of the point, identical): gtsam/base/cholesky.cpp:107-158
-  // (rsqrt + multiplies instead of sqrt + divides: same result to ~1 ulp per operation, a third of the latency)
-  bool ok = v[0] > 0.0;
-  const double i00 = rsqrt(v[0]);
-  const double r00 = v[0] * i00;
-  const double r01 = v[1] * i00, r02 = v[2] * i00;
-  const double p11 = v[3] - r01 * r01;
-  ok = ok && p11 > 0.0;
-  const double i11 = rsqrt(p11);
-  const double r11 = p11 * i11;
-  const double r12 = (v[4] - r01 * r02) * i11;
-  const double p22 = v[5] - r02 * r02 - r12 * r12;
-  ok = ok && p22 > 0.0;
-  const double i22 = rsqrt(p22);
-  const double r22 = p22 * i22;
-  if (!(dexp(r11) - dexp(r22) < 12)) ok = false;
-  if (!STAGED && !live) return;
-  if (live && !ok && sub == 0) atomicMax(&sc->fail_code, INT_MAX - c);
-  const int n = live ? 3 + DC * m + 1 : 0;          // (a point clique of these kinds: one factor per separator camera)
+  const bool hd = hdiag && live;
+  PointFactor f;
+  f.factor(v, lambda, hd ? hdiag : nullptr, hd ? t.didx + t.didx_ptr[c] : nullptr, min_diag, max_diag);
+  if (!live) return;
+  if (!f.ok && sub == 0) atomicMax(&sc->fail_code, INT_MAX - c);
+  const int n = 3 + DC * m + 1;     // (a point clique of these kinds: one factor per separator camera)
   double* M = t.arena + moff;       // compact conditional [R S' d'], column-major 3 x n
-  if (STAGED) {
-    B200_DYN_SMEM(double, sm_dyn);
-    M = sm_dyn + (size_t)(threadIdx.x >> 3) * ncap;     // this point's conditional, staged
-  }
-  if (live && sub == 0) {
-    const double d0 = v[6] * i00;
-    const double d1 = (v[7] - r01 * d0) * i11;
-    const double d2 = (v[8] - r02 * d0 - r12 * d1) * i22;
-    M[0] = r00; M[1] = 0.0; M[2] = 0.0;
-    M[3] = r01; M[4] = r11; M[5] = 0.0;
-    M[6] = r02; M[7] = r12; M[8] = r22;
-    M[3 * (n - 1)] = d0; M[3 * (n - 1) + 1] = d1; M[3 * (n - 1) + 2] = d2;
+  if (sub == 0) {
+    M[0] = f.r00; M[1] = 0.0; M[2] = 0.0;
+    M[3] = f.r01; M[4] = f.r11; M[5] = 0.0;
+    M[6] = f.r02; M[7] = f.r12; M[8] = f.r22;
+    M[3 * (n - 1)] = f.d0; M[3 * (n - 1) + 1] = f.d1; M[3 * (n - 1) + 2] = f.d2;
   }
   if (rec.x >= 0) {
     double* Mc = M + 3 * (3 + tk);
 #pragma unroll
     for (int cc = 0; cc < DC; cc++) {
-      const double w0 = Ap[0][0] * Ac[0][cc] + Ap[1][0] * Ac[1][cc];
-      const double w1 = Ap[0][1] * Ac[0][cc] + Ap[1][1] * Ac[1][cc];
-      const double w2 = Ap[0][2] * Ac[0][cc] + Ap[1][2] * Ac[1][cc];
-      const double s0 = w0 * i00;
-      const double s1 = (w1 - r01 * s0) * i11;
-      const double s2 = (w2 - r02 * s0 - r12 * s1) * i22;
+      double s0, s1, s2;
+      f.s_col(Ap, Ac[0][cc], Ac[1][cc], s0, s1, s2);
       Mc[3 * cc] = s0; Mc[3 * cc + 1] = s1; Mc[3 * cc + 2] = s2;
-    }
-  }
-  if (STAGED) {
-    B200_DYN_SMEM(double, sm_dyn);
-    __syncwarp();
-    const int lane = threadIdx.x & 31;
-#pragma unroll
-    for (int pt = 0; pt < 4; pt++) {
-      const int np = __shfl_sync(0xffffffffu, n, 8 * pt);
-      const int64_t op = __shfl_sync(0xffffffffu, moff, 8 * pt);
-      if (np == 0) continue;       // (warp-uniform: a point past the end of the list)
-      const double* src = sm_dyn + (size_t)((threadIdx.x >> 5) * 4 + pt) * ncap;
-      double* dst = t.arena + op;
-      for (int e = lane; e < 3 * np; e += 32) dst[e] = src[e];
     }
   }
 }
@@ -1015,7 +1026,7 @@ leaf_point_schur_kernel(TreeView t, GroupTable gt, const int* __restrict__ list,
   // is multiplied, and the (dependent) index loads of batch b+2 are in flight behind them.
   const double* srcS[3];       // [S' d'] of the points this warp copies (points warp, warp + nwarp, ... of a batch)
   const JT* srcJ = nullptr;    // this thread's factor (point tid>>3, factor tid&7), staged by camera slot
-  size_t cntJ = 0;
+  int cntJ = 0;
   int slotJ = -1;
   auto load_idx = [&](int b0) {
     const int nb = min(PB, r1 - b0);
@@ -1146,97 +1157,98 @@ __device__ __forceinline__ void dmma_m8n8k4(double& d0, double& d1, double a, do
 #endif
 
 // ---------------------------------------------------------------------------
-// The same per-run half on the FP64 tensor path.  leaf_point_schur_kernel executes about ten thread instructions per useful
-// FMA — the 3x3 register tiles spend their issue slots on shared-memory loads (6 LDS.64 per 9 FMAs) and index arithmetic,
-// not on arithmetic.  Here the run's
-// -S'^T S' is what it is, a SYRK, and so is every camera's [A_c b]^T [A_c b]:
-//   * every WARP runs its own pipeline over mini-batches of 4 points (the run's points are dealt round-robin to the 4
-//     warps): it stages its points' [S' d'] rows TRANSPOSED ([column][k = 3 pt + r], 12 doubles per column: conflict-free
-//     fragments, no padding) and their [A_c b] blocks ([camera][column][k = 2 pt + r]) with cp.async, double-buffered, and
-//     multiplies what it staged — no block barrier in the loop;
+// Both halves of the BAL point leaves in one kernel, the Schur complement on the FP64 tensor path.  One CTA of 4 warps per
+// RUN of points seen by the same cameras; the run's points are dealt to the warps in mini-batches of 4 (warp, warp + 4, ...)
+// and every warp runs its own pipeline over them — no block barrier in the loop:
+//   * it stages the next mini-batch's [A_c b] blocks ([camera][column][k = 2 pt + r]) and A_p ([element][lane]) with
+//     cp.async, double-buffered;
+//   * it factors the current mini-batch's points (PointFactor, lane = point lane>>3, factor lane&7, A_c read column by
+//     column from shared memory) and writes [R S' d'] TRANSPOSED into shared memory ([column][k = 3 pt + r], 12 doubles per
+//     column: conflict-free fragments, no padding); from there every point's conditional leaves as contiguous stores;
 //   * per k-step of 4 rows it loads ONE fragment per 8-column strip and issues mma.sync.m8n8k4.f64 for every tile pair
-//     of the upper triangle (the same fragment is the A operand, negated, and the B operand): 10 DMMAs = 2560 FMAs for
-//     4 shared-memory loads at 32 columns; the (DC+1)^2 block of a camera is one more tile (four at 9 dofs);
+//     of the upper triangle of -S'^T S' (the same fragment is the A operand, negated, and the B operand): 10 DMMAs = 2560
+//     FMAs for 4 shared-memory loads at 32 columns; a camera's (DC+1)^2 block [A_c b]^T [A_c b] is one more tile (four at
+//     9 dofs);
 //   * the four warps' partial sums are added in shared memory in a FIXED order, then one extend-add per entry and run
 //     (HessianFactor::updateHessian of the leaf's separator factor) — a run's contribution is bitwise reproducible.
+// Every operand crosses HBM once: the split path (leaf_point_factor_kernel + leaf_point_schur_kernel) reads the [S' d'] the
+// first kernel has just written and the [A_c b] it has just read a second time.
 // ---------------------------------------------------------------------------
 constexpr int kSmMP = 4;                 // points per warp mini-batch
 constexpr int kSmKS = 3 * kSmMP;         // rows (and pitch) of a staged S'^T column: (q * 12 + g) mod 16 distinct over a half-warp
 constexpr int kSmKA = 2 * kSmMP;         // rows of a staged [A_c b]^T column; pitch 12 (doubles and floats: conflict-free)
 constexpr int kSmPA = 12;
+constexpr int kSmPadA = 4;               // behind every camera's [A_c b]^T block: the 8 cameras of a factor-phase access hit
+                                         // different banks (2 wavefronts per float access instead of 8)
 
+// (min. 3 blocks = 168 registers at 6 dofs and up to 40 columns: at 4 blocks = 128 registers the factorisation spills)
 template <int DC, int NTT, typename JT = double>   // NTT: 8-column strips of the widest separator (+ rhs column) of the kind
-__global__ void __launch_bounds__(128, (NTT <= 4 && DC == 6) ? 4 : ((NTT <= 5 && DC == 6) ? 3 : (NTT <= 7 ? 2 : 1)))
-leaf_point_schur_mma_kernel(TreeView t, GroupTable gt, const int* __restrict__ list, const int* __restrict__ run_ptr,
-                            const int2* __restrict__ pt_tab, const int64_t* __restrict__ pt_off) {
+__global__ void __launch_bounds__(128, (NTT <= 5 && DC == 6) ? 3 : (NTT <= 7 ? 2 : 1))
+leaf_point_fused_mma_kernel(TreeView t, GroupTable gt, const int* __restrict__ list, const int* __restrict__ run_ptr,
+                            const double* __restrict__ lambda_ptr, const double* __restrict__ hdiag, double min_diag,
+                            double max_diag, Scalars* sc, const int2* __restrict__ pt_tab, const int64_t* __restrict__ pt_off) {
   pdl_sync();
   constexpr int MP = kSmMP, KS = kSmKS, PA = kSmPA;
   constexpr int CP = DC < 8 ? 8 : 16, CT = CP / 8;           // [A_c b] has DC + 1 columns: one 8x8 tile, or 2 x 2 at 9 dofs
   constexpr int NAT = CT * (CT + 1) / 2;
-  constexpr int NI = (3 * 8 * NTT + 31) / 32;                // 8-byte copies per lane and point of [S' d']
+  constexpr int SA = CP * PA + kSmPadA;                      // elements per camera of a staged [A_c b]^T
+  constexpr int MC = (8 * NTT - 1) / DC < kPtMaxObs ? (8 * NTT - 1) / DC : kPtMaxObs;   // cameras of the widest separator
   B200_DYN_SMEM(double, sm_dyn);
+  __shared__ int64_t sOff[4][2][MP];                         // per warp and buffer: the points' conditional offsets,
+  __shared__ int sC[4][2][MP];                               // clique ids
+  __shared__ int sSlot[4][2][32];                            // and every lane's camera slot (-1: no factor)
+  const double lambda = *lambda_ptr;
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, g = lane >> 2, q = lane & 3;
+  const int pl = lane >> 3, fl = lane & 7;                   // factorisation: point of the mini-batch, factor slot
   const int r0 = run_ptr[blockIdx.x], r1 = run_ptr[blockIdx.x + 1];
   const int c0 = list[r0];
-  const int p = t.parent[c0];
-  if (p < 0) return;
   const int s = t.ns[c0], w = s + 1;
   const int m = s / DC;                                       // one factor per separator camera
   const int NT = (w + 7) >> 3, WP = 8 * NT;
-  const int s_doubles = 2 * WP * KS;                          // per warp: S'^T, two buffers
-  const int a_elems = 2 * m * CP * PA;                        // per warp: [A_c b]^T of m cameras, two buffers, in JT
-  double* sS = sm_dyn + (size_t)warp * s_doubles;
-  JT* sA = reinterpret_cast<JT*>(sm_dyn + (size_t)4 * s_doubles) + (size_t)warp * a_elems;
+  const int f_doubles = (3 + WP) * KS;                        // per warp: [R S' d']^T of the mini-batch (one buffer)
+  const int a_elems = 2 * m * SA;                             // per warp: [A_c b]^T of m cameras, two buffers, in JT
+  double* sF = sm_dyn + (size_t)warp * f_doubles;
+  double* sS = sF + 3 * KS;                                   // the [S' d'] columns
+  JT* sA = reinterpret_cast<JT*>(sm_dyn + (size_t)4 * f_doubles) + (size_t)warp * (a_elems + 2 * 6 * 32);
+  JT* sP = sA + a_elems;                                      // per warp: A_p, [buffer][element 2 j + r][lane], in JT
   double acc[NTT][NTT][2];                                    // tile (ti <= tj) of -S'^T S'
-  double accA[kPtMaxObs][NAT][2];                             // per camera: tiles of [A_c b]^T [A_c b]
+  double accA[MC][NAT][2];                                    // per camera: tiles of [A_c b]^T [A_c b]
 #pragma unroll
   for (int a = 0; a < NTT; a++)
 #pragma unroll
     for (int b = 0; b < NTT; b++) acc[a][b][0] = acc[a][b][1] = 0.0;
 #pragma unroll
-  for (int ci = 0; ci < kPtMaxObs; ci++)
+  for (int ci = 0; ci < MC; ci++)
 #pragma unroll
     for (int x = 0; x < NAT; x++) accA[ci][x][0] = accA[ci][x][1] = 0.0;
-  // padding never written by the copies: columns behind the rhs column, columns behind b
-  for (int e = lane; e < 2 * WP * KS; e += 32) { const int col = (e / KS) % WP; if (col >= w) sS[e] = 0.0; }
-  for (int e = lane; e < a_elems; e += 32) { const int col = (e / PA) % CP; if (col > DC || e % PA >= kSmKA) sA[e] = (JT)0; }
-  int soff[NI];                                                // destination of this lane's copies, per point + 3 pt
-#pragma unroll
-  for (int i = 0; i < NI; i++) { const int e = lane + 32 * i, col = e / 3; soff[i] = e < 3 * w ? col * KS + (e - 3 * col) : -1; }
+  // padding never written: columns behind the rhs column, columns behind b
+  for (int e = lane; e < f_doubles; e += 32) if (e / KS >= 3 + w) sF[e] = 0.0;
+  for (int e = lane; e < a_elems; e += 32) { const int r = e % SA; if (r / PA > DC || r % PA >= kSmKA) sA[e] = (JT)0; }
   const int npts = r1 - r0, nmb = (npts + MP - 1) / MP;       // mini-batches of the run; this warp takes warp, warp + 4, ...
-  const double* srcS[MP];
   const JT* srcJ = nullptr;      // this lane's factor (point lane>>3 of the mini-batch, factor lane&7), staged by camera slot
-  size_t cntJ = 0;
-  int slotJ = -1;
+  int cntJ = 0;
+  int slotJ = -1, cJ = 0;
+  int64_t offJ = 0;
   auto load_idx = [&](int mb) {
     const int b0 = r0 + MP * mb, nb = min(MP, r1 - b0);
     // one level of index loads (the flat table of the point leaves: engine.cu)
-#pragma unroll
-    for (int z = 0; z < MP; z++) srcS[z] = z < nb ? t.arena + pt_off[b0 + z] + 9 : nullptr;
-    const int pt = lane >> 3, fi = lane & 7;
     slotJ = -1;
-    if (pt < nb) {
-      const int2 rec = pt_tab[(size_t)(b0 + pt) * kPtMaxObs + fi];
+    if (pl < nb) {
+      const int2 rec = pt_tab[(size_t)(b0 + pl) * kPtMaxObs + fl];
+      offJ = pt_off[b0 + pl];
+      cJ = list[b0 + pl];
       if (rec.x >= 0) {
         const GroupView& gv = gt.g[rec.y >> 8];
-        cntJ = (size_t)gv.count;
+        cntJ = (int)gv.count;
         srcJ = reinterpret_cast<const JT*>(gv.J) + rec.x;
         slotJ = rec.y & 0xff;
       }
     }
   };
   auto issue = [&](int buf, int nb) {
-    double* S = sS + buf * WP * KS;
-    JT* A = sA + buf * m * CP * PA;
-#pragma unroll
-    for (int z = 0; z < MP; z++)
-      if (srcS[z]) {
-#pragma unroll
-        for (int i = 0; i < NI; i++)
-          if (soff[i] >= 0) cp_async8(S + soff[i] + 3 * z, srcS[z] + lane + 32 * i);
-      }
+    JT* A = sA + buf * m * SA;
     if (slotJ >= 0) {
-      JT* dst = A + slotJ * CP * PA + 2 * (lane >> 3);
+      JT* dst = A + slotJ * SA + 2 * pl;
 #pragma unroll
       for (int cc = 0; cc < DC; cc++) {
         cp_async_el(dst + cc * PA, srcJ + (size_t)(2 * cc) * cntJ);
@@ -1244,15 +1256,18 @@ leaf_point_schur_mma_kernel(TreeView t, GroupTable gt, const int* __restrict__ l
       }
       cp_async_el(dst + DC * PA, srcJ + (size_t)(2 * (DC + 3)) * cntJ);
       cp_async_el(dst + DC * PA + 1, srcJ + (size_t)(2 * (DC + 3) + 1) * cntJ);
+      JT* P = sP + buf * 6 * 32 + lane;
+#pragma unroll
+      for (int el = 0; el < 6; el++) cp_async_el(P + 32 * el, srcJ + (size_t)(2 * DC + el) * cntJ);
     }
     cp_async_commit();
-    if (nb < MP) {     // a short last mini-batch: the rows of the missing points read as zero
-      for (int e = lane; e < w * (KS - 3 * nb); e += 32) { const int col = e / (KS - 3 * nb); S[col * KS + 3 * nb + (e - col * (KS - 3 * nb))] = 0.0; }
+    sSlot[warp][buf][lane] = slotJ;
+    if (fl == 0 && pl < nb) { sOff[warp][buf][pl] = offJ; sC[warp][buf][pl] = cJ; }
+    if (nb < MP)       // a short last mini-batch: the rows of the missing points read as zero
       for (int e = lane; e < m * (DC + 1) * (kSmKA - 2 * nb); e += 32) {
         const int cc = e / (kSmKA - 2 * nb);
-        A[cc / (DC + 1) * CP * PA + cc % (DC + 1) * PA + 2 * nb + (e - cc * (kSmKA - 2 * nb))] = (JT)0;
+        A[cc / (DC + 1) * SA + cc % (DC + 1) * PA + 2 * nb + (e - cc * (kSmKA - 2 * nb))] = (JT)0;
       }
-    }
   };
   if (warp < nmb) {
     load_idx(warp);
@@ -1261,35 +1276,85 @@ leaf_point_schur_mma_kernel(TreeView t, GroupTable gt, const int* __restrict__ l
   }
   int buf = 0;
   for (int mb = warp; mb < nmb; mb += 4, buf ^= 1) {
+    const int nb = min(MP, npts - MP * mb);
     if (mb + 4 < nmb) {
       issue(buf ^ 1, min(MP, npts - MP * (mb + 4)));
-      if (mb + 8 < nmb) load_idx(mb + 8);
       cp_async_wait<1>();
     } else {
       cp_async_wait<0>();
     }
     __syncwarp();
-    const double* S = sS + buf * WP * KS;
+    const JT* A = sA + buf * m * SA;
+    {   // ---- the mini-batch's points: factor, [R S' d'] into sF; the rows of missing points are zero ----
+      const int slot = sSlot[warp][buf][lane];
+      const bool live = pl < nb;
+      const JT* Al = A + slot * SA + 2 * pl;                  // this lane's [A_c b]^T (slot >= 0)
+      double Ap[2][3], v[9];
+#pragma unroll
+      for (int i = 0; i < 9; i++) v[i] = 0.0;
+      if (slot >= 0) {
+        const JT* P = sP + buf * 6 * 32 + lane;
+#pragma unroll
+        for (int j = 0; j < 3; j++) { Ap[0][j] = (double)P[32 * (2 * j)]; Ap[1][j] = (double)P[32 * (2 * j + 1)]; }
+        const double b[2] = {(double)Al[DC * PA], (double)Al[DC * PA + 1]};
+        PointFactor::lane_terms(Ap, b, v);
+      }
+      const int c = live ? sC[warp][buf][pl] : 0;
+      const bool hd = hdiag && live;
+      PointFactor f;
+      f.factor(v, lambda, hd ? hdiag : nullptr, hd ? t.didx + t.didx_ptr[c] : nullptr, min_diag, max_diag);
+      if (live) {
+        if (fl == 0) {
+          if (!f.ok) atomicMax(&sc->fail_code, INT_MAX - c);
+          double* F = sF + 3 * pl;
+          F[0] = f.r00; F[1] = 0.0; F[2] = 0.0;
+          F[KS] = f.r01; F[KS + 1] = f.r11; F[KS + 2] = 0.0;
+          F[2 * KS] = f.r02; F[2 * KS + 1] = f.r12; F[2 * KS + 2] = f.r22;
+          F[(3 + s) * KS] = f.d0; F[(3 + s) * KS + 1] = f.d1; F[(3 + s) * KS + 2] = f.d2;
+        }
+        if (slot >= 0) {
+          double* F = sS + DC * slot * KS + 3 * pl;
+#pragma unroll
+          for (int cc = 0; cc < DC; cc++) {
+            double s0, s1, s2;
+            f.s_col(Ap, (double)Al[cc * PA], (double)Al[cc * PA + 1], s0, s1, s2);
+            F[cc * KS] = s0; F[cc * KS + 1] = s1; F[cc * KS + 2] = s2;
+          }
+        }
+      } else {
+        for (int col = fl; col < w; col += 8) { double* F = sS + col * KS + 3 * pl; F[0] = F[1] = F[2] = 0.0; }
+      }
+    }
+    __syncwarp();
+    // ---- every point's conditional [R S' d'] (column-major 3 x (3 + w)) leaves as contiguous stores ----
+#pragma unroll 1
+    for (int z = 0; z < nb; z++) {
+      double* dst = t.arena + sOff[warp][buf][z];
+      const double* src = sF + 3 * z;
+#pragma unroll 1
+      for (int e = lane; e < 3 * (3 + w); e += 32) { const int col = e / 3; dst[e] = src[col * KS + (e - 3 * col)]; }
+    }
+    if (mb + 8 < nmb) load_idx(mb + 8);      // (here, not next to issue(): the factorisation's registers are free again)
+    // ---- the mini-batch's share of the run's Schur complement ----
 #pragma unroll
     for (int k4 = 0; k4 < KS / 4; k4++) {
-      double f[NTT];
+      double fr[NTT];
 #pragma unroll
-      for (int a = 0; a < NTT; a++) f[a] = a < NT ? S[(8 * a + g) * KS + 4 * k4 + q] : 0.0;
+      for (int a = 0; a < NTT; a++) fr[a] = a < NT ? sS[(8 * a + g) * KS + 4 * k4 + q] : 0.0;
 #pragma unroll
       for (int a = 0; a < NTT; a++)
 #pragma unroll
         for (int b = a; b < NTT; b++)
-          if (b < NT) dmma_m8n8k4(acc[a][b][0], acc[a][b][1], -f[a], f[b]);     // (warp-uniform)
+          if (b < NT) dmma_m8n8k4(acc[a][b][0], acc[a][b][1], -fr[a], fr[b]);     // (warp-uniform)
     }
-    const JT* A = sA + buf * m * CP * PA;
 #pragma unroll
-    for (int ci = 0; ci < kPtMaxObs; ci++) {
+    for (int ci = 0; ci < MC; ci++) {
       if (ci >= m) break;
 #pragma unroll
       for (int k4 = 0; k4 < kSmKA / 4; k4++) {
         double fa[CT];
 #pragma unroll
-        for (int x = 0; x < CT; x++) fa[x] = (double)A[(ci * CP + 8 * x + g) * PA + 4 * k4 + q];
+        for (int x = 0; x < CT; x++) fa[x] = (double)A[ci * SA + (8 * x + g) * PA + 4 * k4 + q];
 #pragma unroll
         for (int x = 0; x < CT; x++)
 #pragma unroll
@@ -1298,9 +1363,11 @@ leaf_point_schur_mma_kernel(TreeView t, GroupTable gt, const int* __restrict__ l
     }
     __syncwarp();
   }
+  const int p = t.parent[c0];
+  if (p < 0) return;      // a root point clique: factored, nothing to extend-add into (block-uniform)
   // ---- the four warps' sums, added in a fixed order in shared memory (the staging buffers are free now) ----
   __syncthreads();
-  double* R = sm_dyn;                                          // [WP][WP], upper triangle used (WP^2 <= 96 WP doubles of S' staging)
+  double* R = sm_dyn;                                          // [WP][WP], upper triangle used (the launch sizes it)
   for (int round = 0; round < 4; round++) {
     if (warp == round) {
 #pragma unroll
@@ -1316,7 +1383,7 @@ leaf_point_schur_mma_kernel(TreeView t, GroupTable gt, const int* __restrict__ l
           }
       __syncwarp();
 #pragma unroll
-      for (int ci = 0; ci < kPtMaxObs; ci++) {
+      for (int ci = 0; ci < MC; ci++) {
         if (ci >= m) break;
 #pragma unroll
         for (int x = 0; x < CT; x++)

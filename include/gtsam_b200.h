@@ -259,10 +259,11 @@ int b200_get_jacobians(b200_problem* prob, int64_t group, double* out);
 int b200_set_jacobian_precision(b200_problem* prob, int fp32);
 int b200_get_jacobian_precision(const b200_problem* prob);
 /* Kernel-variant switches of one problem, for A/B measurements (every variant computes the same result):
- * "schur_mma" 1 (default) = the per-run Schur complement of the BAL point leaves on the FP64 tensor path, 0 = the
- * FMA-tile kernel; "schur_pb" 4 / 6 = its points per staged batch; "df_minb" 2 / 3 = the dense-front kernel variant;
- * "lin_variant" 0 / 4 = linearize_kernel build of the projection groups (64 / 128 registers); "factor_staged" 1 (default) / 0
- * = leaf_point_factor_kernel stores the conditionals through shared memory / directly.  Unknown key: B200_INVALID_ARGUMENT. */
+ * "schur_mma" 1 (default) = the BAL point leaves are factored and their per-run Schur complement formed on the FP64
+ * tensor path in one kernel, 0 = a per-point factor kernel followed by the FMA-tile Schur kernel; "schur_pb" 4 / 6 = the
+ * latter's points per staged batch; "df_minb" 2 / 3 = the dense-front kernel variant; "lin_variant" 0 / 4 =
+ * linearize_kernel build of the projection groups (64 / 128 registers); "factor_staged" is accepted and has no effect
+ * (kept so that existing callers still succeed).  Unknown key: B200_INVALID_ARGUMENT. */
 int b200_set_tuning(b200_problem* prob, const char* key, int64_t value);
 
 /* GaussianFactorGraph::hessianDiagonal(), gtsam/linear/GaussianFactorGraph.cpp:279-287.
