@@ -395,44 +395,6 @@ static int enqueue_solve(b200_problem* p, bool damped, int diagonal, double min_
                                                                p->max_small_n, p->d_scalars);
       ctx->launches++;
     }
-    if (L.large_count) {
-      PhaseScope ps(p, PH_ELIM_LARGE);
-      const int* list = p->d_lvl_large + L.large_begin;
-      const int fuse = p->fuse_ea ? 1 : 0;          // last update of a front extend-adds straight into the parent
-      const bool big = L.large_max_n >= p->big_min_n;   // big fronts: one K=128 trailing update per 128 columns
-      auto tiles = [](int rows, int cols, int T) {   // upper-trapezoid tile count
-        const int TR = (rows + T - 1) / T, TC = (cols + T - 1) / T;
-        int cnt = 0;
-        for (int ti = 0; ti < TR; ti++) cnt += std::max(0, TC - ti);
-        return std::max(1, cnt);
-      };
-      for (int K0 = 0; K0 < L.large_max_nf; K0 += kBig) {
-        for (int k0 = K0; k0 < std::min(K0 + kBig, L.large_max_nf); k0 += kNB) {
-          const int ncol = L.large_max_n - k0 - 1;
-          launch_k(panel_kernel, dim3(dim3(std::max(1, (ncol + kTrsmCols - 1) / kTrsmCols), L.large_count)), dim3(kTrsmCols), 0, st, 
-              t, list, k0, p->d_scalars, p->d_rdiag);
-          if (!big) {
-            launch_k(update_kernel<64, 4, 32>, dim3(dim3(tiles(ncol, ncol, 64), L.large_count)), dim3(256), 0, st, t, list, 0, K0, k0, p->d_rdiag, fuse);
-          } else {
-            const int rows = std::min(K0 + kBig, L.large_max_nf) - k0 - 1;
-            launch_k(update_kernel<64, 4, 32>, dim3(dim3(tiles(std::max(rows, 1), ncol, 64), L.large_count)), dim3(256), 0, st, t, list, 1, K0, k0, p->d_rdiag, fuse);
-          }
-          ctx->launches += 2;
-        }
-        if (big) {
-          const int m = L.large_max_n - K0 - 1;
-          if (p->use_dmma) launch_k(update_dmma_kernel, dim3(dim3(tiles(m, m, 128), L.large_count)), dim3(256), 0, st, t, list, K0, fuse);
-          else launch_k(update_kernel<128, 8, 16>, dim3(dim3(tiles(m, m, 128), L.large_count)), dim3(256), 0, st, t, list, 2, K0, 0, p->d_rdiag, fuse);
-          ctx->launches++;
-        }
-      }
-      if (!fuse) {
-        const int64_t w = L.large_max_ns + 1;
-        const int gx = (int)std::min<int64_t>((w * w + 255) / 256, 4096);
-        launch_k(extend_add_kernel, dim3(dim3(gx, L.large_count)), dim3(256), 0, st, t, list);
-        ctx->launches++;
-      }
-    }
   }
   // ---- back-substitution, roots to leaves ----
   if (p->n_bs_flags) B200_CUDA(cudaMemsetAsync(p->d_bs_flags, 0, (size_t)p->n_bs_flags * sizeof(int), st));
@@ -1091,8 +1053,8 @@ int b200_problem_destroy(b200_problem* p) {
   cudaFree(p->d_val_off); cudaFree(p->d_var_type); cudaFree(p->d_var_dof); cudaFree(p->d_cal); cudaFree(p->d_arena);
   cudaFree(p->d_off); cudaFree(p->d_nf); cudaFree(p->d_ns); cudaFree(p->d_parent); cudaFree(p->d_ea_ptr);
   cudaFree(p->d_didx_ptr); cudaFree(p->d_ea_map); cudaFree(p->d_didx); cudaFree(p->d_diag_index);
-  cudaFree(p->d_lvl_small); cudaFree(p->d_lvl_large); cudaFree(p->d_lvl_bsmall); cudaFree(p->d_lvl_blarge); cudaFree(p->d_marg_work); cudaFree(p->d_marg_path); cudaFree(p->d_marg_out); cudaFree(p->d_lvl_bpoint); cudaFree(p->d_ld);
-  cudaFree(p->d_rdiag); cudaFree(p->d_bs_flags); cudaFree(p->d_bs_flag_base);
+  cudaFree(p->d_lvl_small); cudaFree(p->d_lvl_bsmall); cudaFree(p->d_lvl_blarge); cudaFree(p->d_marg_work); cudaFree(p->d_marg_path); cudaFree(p->d_marg_out); cudaFree(p->d_lvl_bpoint); cudaFree(p->d_ld);
+  cudaFree(p->d_bs_flags); cudaFree(p->d_bs_flag_base);
   cudaFree(p->d_df_tasks[0]); cudaFree(p->d_df_tasks[1]); cudaFree(p->d_df_flag_off); cudaFree(p->d_df_expect); cudaFree(p->d_df_sync); cudaFree(p->d_df_trace);
   cudaFree(p->d_winv); cudaFree(p->d_winv_off); cudaFree(p->d_red);
   cudaFree(p->d_view_idx[0]); cudaFree(p->d_view_idx[1]); cudaFree(p->d_view_buf); cudaFree(p->d_gather_buf);
@@ -1173,7 +1135,7 @@ static int create_problem(b200_ctx* ctx, const b200_problem_desc* d, const b200_
   std::vector<int> clique_owner, factor_owner, top_owner;
   shard_plan(S, ngroups, total, ctx->world, &fused, &is_top, &clique_owner, &factor_owner, /*allow_leaf=*/d != nullptr, &top_owner);
   const int rank = ctx->rank;
-  p->top_staged = ctx->world > 1 && getenv("B200_REPLICATED_TOP") == nullptr && getenv("B200_LEGACY_FRONTS") == nullptr;
+  p->top_staged = ctx->world > 1 && getenv("B200_REPLICATED_TOP") == nullptr;
   std::vector<int> fused_list;   // the fused leaf cliques THIS rank owns
   for (int64_t c = 0; c < S.ncliques; c++)
     if (fused[c] && clique_owner[c] == rank) fused_list.push_back((int)c);
@@ -1256,9 +1218,6 @@ static int create_problem(b200_ctx* ctx, const b200_problem_desc* d, const b200_
   }
   lap("shard plan + leaf runs");
   p->n_fused = (int)fused_list.size();
-  p->big_min_n = getenv("B200_BIG_MIN_N") ? atoi(getenv("B200_BIG_MIN_N")) : 1024;
-  p->use_dmma = getenv("B200_NO_DMMA") == nullptr;
-  p->fuse_ea = getenv("B200_NO_FUSE_EA") == nullptr;
   p->schur_pb = (getenv("B200_SCHUR_PB") && atoi(getenv("B200_SCHUR_PB")) == 6) ? 6 : 4;
   p->schur_mma = !(getenv("B200_SCHUR_MMA") && atoi(getenv("B200_SCHUR_MMA")) == 0);
   if (getenv("B200_LIN_VARIANT")) p->lin_variant = atoi(getenv("B200_LIN_VARIANT"));
@@ -1468,36 +1427,32 @@ static int create_problem(b200_ctx* ctx, const b200_problem_desc* d, const b200_
     }
   }
   lap("leaf factor lists + point table");
-  // ---- level plans: small (one warp per clique) / large (blocked) ----
+  // ---- level plans: small (one warp per clique) / tile dataflow ----
   // phase 0: the subtrees this rank owns, leaves to subtree roots; phase 1: the replicated top.
   // p->levels = [phase-0 levels ..., phase-1 levels ...]; elimination walks it forwards (with the
   // all-reduce of the top fronts between the phases), back-substitution walks it backwards.
-  std::vector<int> small, large, bsmall, blarge, bpoint;
+  std::vector<int> small, bsmall, blarge, bpoint;
   p->levels.resize(2 * S.nlevels);
   p->n_sub_levels = (int)S.nlevels;
   p->max_small_n = 1;
-  p->use_df = getenv("B200_LEGACY_FRONTS") == nullptr;
   // tile dataflow (front_df.cuh): per phase, from the first level that holds a front wider than kSmallMaxN upwards,
   // every non-leaf front is a set of tiles of ONE launch; the levels below it (small fronts only) keep elim_small_kernel
   int df_first[2] = {INT_MAX, INT_MAX};
   std::vector<int4> df_tasks[2];
   std::vector<int> df_flag_off(S.ncliques, 0), df_expect(S.ncliques, 0), df_tiles(S.ncliques, 0);
   int64_t df_nflags = 0;
-  if (!p->use_df) p->top_staged = false;
   auto in_phase = [&](int phase, int c) {
     return phase == 0 ? (!is_top[c] && clique_owner[c] == rank) : (is_top[c] != 0 && (!p->top_staged || top_owner[c] == rank));
   };
-  if (p->use_df)
-    for (int phase = 0; phase < 2; phase++)
-      for (int64_t c = 0; c < S.ncliques; c++)
-        if (in_phase(phase, (int)c) && !fused[c] && S.nf[c] + S.ns[c] + 1 > kSmallMaxN) df_first[phase] = std::min(df_first[phase], S.level[c]);
+  for (int phase = 0; phase < 2; phase++)
+    for (int64_t c = 0; c < S.ncliques; c++)
+      if (in_phase(phase, (int)c) && !fused[c] && S.nf[c] + S.ns[c] + 1 > kSmallMaxN) df_first[phase] = std::min(df_first[phase], S.level[c]);
   if (p->top_staged) df_first[1] = 0;     // every top front goes through its stage's reduce + dataflow launch
   for (int phase = 0; phase < 2; phase++)
   for (int64_t l = 0; l < S.nlevels; l++) {
     LevelPlan& L = p->levels[phase * S.nlevels + l];
     L = LevelPlan();
     L.small_begin = (int)small.size();
-    L.large_begin = (int)large.size();
     L.bsmall_begin = (int)bsmall.size();
     L.blarge_begin = (int)blarge.size();
     std::vector<int> pts[2];
@@ -1516,21 +1471,15 @@ static int create_problem(b200_ctx* ctx, const b200_problem_desc* d, const b200_
         bsmall.push_back(c);
         p->max_small_n = std::max(p->max_small_n, nn);
       } else {
-        if (l >= df_first[phase]) {
-          // tiles (column block j, row tile r) of the upper trapezoid, ticket order: column-major (dependencies point backwards)
-          const int K = (S.nf[c] + kDfB - 1) / kDfB, NB = K + (nn - S.nf[c] + kDfB - 1) / kDfB;
-          if (p->df_level[phase] < 0) p->df_level[phase] = (int)(phase * S.nlevels + l);
-          df_flag_off[c] = (int)df_nflags;
-          df_nflags += (int64_t)K * NB;
-          for (int j = 0; j < NB; j++)
-            for (int r = 0; kDfTR * r <= j; r++) { df_tasks[phase].push_back(make_int4(c, j, r, 0)); df_tiles[c]++; }
-          if (S.parent[c] >= 0) df_expect[S.parent[c]] += df_tiles[c];
-        } else {
-        large.push_back(c);
-        L.large_max_nf = std::max(L.large_max_nf, S.nf[c]);
-        L.large_max_ns = std::max(L.large_max_ns, S.ns[c]);
-        L.large_max_n = std::max(L.large_max_n, nn);
-        }
+        if (l < df_first[phase]) FAIL(B200_INVALID_ARGUMENT, "level plan: a front wider than kSmallMaxN below the first dataflow level (internal)");
+        // tiles (column block j, row tile r) of the upper trapezoid, ticket order: column-major (dependencies point backwards)
+        const int K = (S.nf[c] + kDfB - 1) / kDfB, NB = K + (nn - S.nf[c] + kDfB - 1) / kDfB;
+        if (p->df_level[phase] < 0) p->df_level[phase] = (int)(phase * S.nlevels + l);
+        df_flag_off[c] = (int)df_nflags;
+        df_nflags += (int64_t)K * NB;
+        for (int j = 0; j < NB; j++)
+          for (int r = 0; kDfTR * r <= j; r++) { df_tasks[phase].push_back(make_int4(c, j, r, 0)); df_tiles[c]++; }
+        if (S.parent[c] >= 0) df_expect[S.parent[c]] += df_tiles[c];
         if (nn <= kSmallMaxN) { bsmall.push_back(c); continue; }
         // back-substitution cares about the pivots only: thin fronts (<= 8 pivots: one pass of the one-warp kernel
         // over the separator) skip the multi-CTA flag machinery (faster on the BAL trees, about even on sphere2500)
@@ -1546,7 +1495,6 @@ static int create_problem(b200_ctx* ctx, const b200_problem_desc* d, const b200_
     }
     L.small_count = (int)small.size() - L.small_begin;
     L.bsmall_count = (int)bsmall.size() - L.bsmall_begin;
-    L.large_count = (int)large.size() - L.large_begin;
     // ticket order inside a level: by column block first, across ALL the level's fronts (then front, row tile).  A tile of column
     // j has nothing to wait for once pivot step j is over, so the resident CTAs (2-3 per SM) are the columns next to every front's
     // pivot — the tiles with work — instead of all the columns of the first few fronts parked on their dependencies while the other
@@ -1672,6 +1620,9 @@ static int create_problem(b200_ctx* ctx, const b200_problem_desc* d, const b200_
     p->df_ntasks[phase] = (int)df_tasks[phase].size();
     if (p->df_ntasks[phase]) UP(upload(&p->d_df_tasks[phase], df_tasks[phase], st));
   }
+  // backsub_large_kernel solves with the diagonal-block inverses W that front_df_kernel leaves behind
+  for (int c : blarge)
+    if (!df_tiles[c]) FAIL(B200_INVALID_ARGUMENT, "level plan: a multi-CTA back-substitution front without diagonal-block inverses (internal)");
   if (p->df_ntasks[0] + p->df_ntasks[1]) {
     std::vector<int64_t> woff(S.ncliques, -1);
     int64_t wtot = 0;
@@ -1698,7 +1649,6 @@ static int create_problem(b200_ctx* ctx, const b200_problem_desc* d, const b200_
   }
   UP(upload(&p->d_lvl_small, small, st));
   UP(upload(&p->d_lvl_bsmall, bsmall, st));
-  UP(upload(&p->d_lvl_large, large, st));
   UP(upload(&p->d_lvl_blarge, blarge, st));
   UP(upload(&p->d_lvl_bpoint, bpoint, st));
   {
@@ -1708,11 +1658,6 @@ static int create_problem(b200_ctx* ctx, const b200_problem_desc* d, const b200_
     p->n_bs_flags = fbase.back();
     B200_CUDA(cudaMalloc((void**)&p->d_bs_flags, (size_t)std::max(1, fbase.back()) * sizeof(int)));
     B200_CUDA(cudaMemsetAsync(p->d_bs_flags, 0, (size_t)std::max(1, fbase.back()) * sizeof(int), st));
-  }
-  {
-    int maxl = 1;
-    for (auto& L : p->levels) maxl = std::max(maxl, L.large_count);
-    B200_CUDA(cudaMalloc((void**)&p->d_rdiag, (size_t)maxl * kNB * kNB * sizeof(double)));
   }
   lap("level plans + dataflow tickets");
   // ---- values views (sharded problems move only what a rank needs / owns between host and device) ----

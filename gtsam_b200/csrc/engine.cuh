@@ -82,9 +82,6 @@ struct Scalars {           // device scalars fetched once per LM try
 struct LevelPlan {
   int small_begin, small_count;   // range in d_lvl_small (elimination, one warp per clique)
   int bsmall_begin, bsmall_count; // range in d_lvl_bsmall (back-substitution, one warp per clique: at most kSmallMaxN pivots)
-  int large_begin, large_count;   // range in d_lvl_large
-  int large_max_nf, large_max_n;  // over the large cliques of the level
-  int large_max_ns;
   int blarge_begin, blarge_count; // back-substitution of fronts with more than kSmallMaxN pivots (range in d_lvl_blarge)
   int blarge_max_nf;
   int bpoint_begin[2], bpoint_count[2];  // BAL point leaves, DC = 6 / 9 (ranges in d_lvl_bpoint)
@@ -142,8 +139,6 @@ struct b200_problem {
   std::vector<int64_t> h_off;       // final arena offsets (fused leaves store f x n only)
   std::vector<int> h_ld;
   // fused leaf path
-  int big_min_n = 1024;   // fronts at least this large use the 128-column big-panel scheme
-  bool use_dmma = true;   // trailing update of big fronts on the FP64 tensor path (DMMA)
   int n_fused = 0, n_runs = 0, leaf_lb_cap = 1, leaf_acc_cap = 0;
   int leaf_run_begin[3] = {0, 0, 0}, leaf_run_end[3] = {0, 0, 0};  // run ranges: generic / point DC=6 / point DC=9
   int schur_pb = 4;                                                 // points per staged batch of leaf_point_schur_kernel
@@ -161,7 +156,7 @@ struct b200_problem {
   int64_t *d_ea_ptr = nullptr, *d_didx_ptr = nullptr;
   int *d_ea_map = nullptr, *d_didx = nullptr;
   int64_t* d_diag_index = nullptr;  // per delta scalar: arena index of its diagonal entry
-  int *d_lvl_small = nullptr, *d_lvl_large = nullptr, *d_lvl_bsmall = nullptr, *d_lvl_blarge = nullptr, *d_lvl_bpoint = nullptr;
+  int *d_lvl_small = nullptr, *d_lvl_bsmall = nullptr, *d_lvl_blarge = nullptr, *d_lvl_bpoint = nullptr;
   std::vector<b200::LevelPlan> levels;
   int *d_bs_flags = nullptr, *d_bs_flag_base = nullptr;  // publish flags of the multi-CTA back-substitution
   int n_bs_flags = 0;
@@ -171,10 +166,7 @@ struct b200_problem {
   double graph_min_diag[2] = {0, 0}, graph_max_diag[2] = {0, 0};
   bool hdiag_valid = false;         // d_hdiag holds hessianDiagonal of the current linearization
   int64_t try_launches = 0;
-  bool fuse_ea = true;              // fold extend_add_kernel into each front's last update
-  double* d_rdiag = nullptr;        // factored diagonal blocks published by panel_kernel
   // tile-dataflow elimination of the non-leaf fronts (front_df.cuh): one launch per phase (own subtrees / replicated top)
-  bool use_df = true;
   int df_level[2] = {-1, -1};       // index in `levels` at which the launch of the phase is issued
   int df_ntasks[2] = {0, 0};
   int4* d_df_tasks[2] = {nullptr, nullptr};

@@ -257,18 +257,11 @@ def edge(_):
 
 
 def bigfront(_):
-    """tests/test_gpu_parity.py::test_big_front_scheme_matches_oracle: the 128-column big-panel scheme with the DMMA
-    trailing update (emulated fragment layout) and with the FP64-FMA tile kernel, forced onto mid-size fronts."""
+    """Fronts of 128 columns and more through both builds of the tile dataflow (front_df_kernel<2> / <3>, emulated DMMA
+    fragment layout), against the oracle."""
     from gtsam_b200 import datasets
-    for legacy, no_dmma, minb in ((True, False, 0), (True, True, 0), (False, False, 2), (False, False, 3)):   # last two: the tile dataflow (front_df_kernel<2> / <3>), the default
-        os.environ.pop("B200_LEGACY_FRONTS", None); os.environ.pop("B200_DF_MINB", None)
-        if legacy:
-            os.environ["B200_LEGACY_FRONTS"] = "1"
-        if minb:
-            os.environ["B200_DF_MINB"] = str(minb)
-        os.environ["B200_BIG_MIN_N"] = "64"
-        if no_dmma:
-            os.environ["B200_NO_DMMA"] = "1"
+    for minb in (2, 3):
+        os.environ["B200_DF_MINB"] = str(minb)
         prob = datasets.make("sphere_tiny", layers=10, per_ring=16)
         dev, orc = capi.DeviceProblem(ctx, prob), O.OracleProblem(prob)
         info = dev.symbolic_info()
@@ -281,7 +274,7 @@ def bigfront(_):
         a, b = dev.conditional(info.ncliques - 1), orc.conditional(info.ncliques - 1)
         assert np.abs(a - b).max() <= 1e-7 * max(1.0, np.abs(b).max())
         dev.close()
-    os.environ.pop("B200_BIG_MIN_N", None); os.environ.pop("B200_NO_DMMA", None); os.environ.pop("B200_DF_MINB", None)
+    os.environ.pop("B200_DF_MINB", None)
 
 
 def midsize(model):
@@ -321,7 +314,7 @@ def midsize(model):
 def coverage(_):
     """Kernel instantiations no fixture reaches (tests/emu/kernel_coverage.py): PriorFactor<Point3> outside the fused
     leaves (points ordered LAST, so their cliques are interior), Dogleg with FP32 Jacobian storage on every factor family
-    (gradient_kernel<T, float>), the separate extend-add of the large fronts (B200_NO_FUSE_EA)."""
+    (gradient_kernel<T, float>)."""
     from gtsam_b200 import datasets
     b = datasets.make("bal_tiny", ncams=8, npoints=40, visibility="scattered")
     pts = np.where(b.var_type == P.VAR_POINT3)[0][:10]
@@ -434,14 +427,6 @@ def coverage(_):
                 dev.close()
         finally:
             os.environ.pop("B200_DF_ORDER"); os.environ.pop("B200_DF_LAG")
-    os.environ["B200_NO_FUSE_EA"] = "1"; os.environ["B200_LEGACY_FRONTS"] = "1"   # the level-by-level panel / update chain
-    try:
-        prob = util.load_case("sphere_small_colamd")
-        dev = capi.DeviceProblem(ctx, prob)
-        util.check_against_dump(dev, prob, util.golden("sphere_small_colamd", "dump1"), 1e-2, 1)
-        dev.close()
-    finally:
-        os.environ.pop("B200_NO_FUSE_EA"); os.environ.pop("B200_LEGACY_FRONTS")
 
 
 SCEN = dict(coverage=coverage, midsize=midsize, edge=edge, bigfront=bigfront, gnc=gnc_scenario, typed=typed, fp32=fp32, linear=linear, marginals=marginals, dogleg=dogleg, gn=gn, mirror=linear_mirror)

@@ -308,29 +308,3 @@ def test_tile_dataflow_fronts_match_oracle(gpu_ctx):
             worst = max(worst, np.abs(a - b).max() / max(1.0, np.abs(b).max()))
         assert worst <= 1e-7, worst
         dev.close()
-
-
-@pytest.mark.parametrize("no_dmma", [False, True])
-def test_big_front_scheme_matches_oracle(gpu_ctx, monkeypatch, no_dmma):
-    """Fronts >= 1024 use 128-column big panels (band updates + one K=128 trailing update, on the
-    FP64 tensor path: mma.sync m8n8k4 f64 / DMMA).  Force that scheme on mid-size fronts
-    (B200_BIG_MIN_N) so it is covered at a size the oracle finishes in seconds."""
-    monkeypatch.setenv("B200_BIG_MIN_N", "64")
-    monkeypatch.setenv("B200_LEGACY_FRONTS", "1")     # the level-by-level panel / update chain of round 1 (kept for A/B)
-    if no_dmma:
-        monkeypatch.setenv("B200_NO_DMMA", "1")
-    for kw in (dict(layers=14, per_ring=24), dict(layers=14, per_ring=24, ordering="reverse")):
-        prob = datasets.make("sphere_tiny", **kw)
-        dev, orc = capi.DeviceProblem(gpu_ctx, prob), O.OracleProblem(prob)
-        assert dev.symbolic_info().max_frontal_dim + dev.symbolic_info().max_separator_dim >= 256
-        dev.linearize(); orc.linearize()
-        for lam in (0.0, 1e-3):
-            st, e0, e1, _ = dev.solve(lam)
-            so, f0, f1, _ = orc.solve(lam)
-            assert st == so == 0
-            assert util.rel2(dev.get_delta(), orc.get_delta()) <= 1e-8
-            assert abs(e1 - f1) <= 1e-9 * f0
-        info = dev.symbolic_info()
-        a, b = dev.conditional(info.ncliques - 1), orc.conditional(info.ncliques - 1)
-        assert np.abs(a - b).max() <= 1e-7 * max(1.0, np.abs(b).max())
-        dev.close()

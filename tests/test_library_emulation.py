@@ -7,7 +7,7 @@ golden vectors of the unmodified reference.
 It is how the code written after this round's GPU budget was spent gets exercised end to end before its first hardware
 run: the GaussianFactorGraph level (JacobianFactor / HessianFactor groups), the FP32-storage mode through the float
 instantiations of the leaf kernels (cp.async staging included), the Pose2 factor family, METIS-ordered BAL, the joint
-marginal kernel — next to paths that are also validated on the GPU (the BAL point-leaf kernels, the panel / update chain,
+marginal kernel — next to paths that are also validated on the GPU (the BAL point-leaf kernels, the tile-dataflow fronts,
 the flag-chained back-substitution, Dogleg, Gauss-Newton, LM), which makes the emulation itself credible.  It checks
 logic and arithmetic, not the GPU: no memory-model subtleties, no performance.  The scenario groups run as parallel
 processes (tests/emu/run_scenarios.py).
@@ -40,7 +40,7 @@ GROUPS = [
     # FP32-storage mode (float instantiations, cp.async staging of floats in the point-leaf Schur kernel)
     ["fp32:bal_tiny_s2", "fp32:bal_tiny_bundler", "fp32:bal_small_metis", "fp32:sphere_tiny_gaussian", "fp32:pose2_ring", "fp32:pose2_ring_colamd",
      "marginals:bal_tiny_s2", "marginals:sphere_tiny", "marginals:bal_tiny_bundler", "marginals:pose2_ring"],
-    # degenerate shapes + API misuse; the big-panel scheme (DMMA fragment layout emulated) forced onto mid-size fronts
+    # degenerate shapes + API misuse; fronts of 128+ columns through both tile-dataflow builds (DMMA fragment layout emulated)
     # ... and long runs of points per CTA (several cp.async batches, both batch sizes, 2 and 3 tiles per thread) in both storage modes
     # coverage: instantiations no fixture reaches (tests/emu/kernel_coverage.py lists what is left)
     ["edge:x", "coverage:x", "midsize:cal3_s2", "midsize:bundler", "midsize:bundler@8", "midsize:cal3_s2@8", "midsize:bundler@4", "midsize:cal3_s2@5", "midsize:bundler@3", "bigfront:x"],
