@@ -311,6 +311,31 @@ def midsize(model):
         dev.close()
 
 
+def leafshapes(model):
+    """A mixed-shape BAL build of tests/test_point_leaf_shapes.py (fast-path points at every m, runs of 1 to 17 points,
+    the generic leaves next to them), cal3_s2 up to 8 observations per point (<6, 7>) or bundler up to 4 (<9, 5>), FP64 and
+    FP32 storage: the factorisation and back-substitution against that file's extended-precision backward-error checks."""
+    import test_point_leaf_shapes as T
+    m_max = 8 if model == "cal3_s2" else 4
+    prob = T.mixed_bal(model, m_max, counts=T.SMALL_COUNTS)
+    for f32 in (False, True):
+        os.environ["B200_LEAF_RUN_MAX"] = "17"
+        try:
+            dev = capi.DeviceProblem(ctx, prob)
+        finally:
+            os.environ.pop("B200_LEAF_RUN_MAX")
+        dev.set_jacobian_precision(f32)
+        dev.linearize()
+        for lam, diag in ((1e-2, False), (1e-3, True)):
+            st, e0, e1, _ = dev.solve(lam, diag)
+            assert st == 0
+            rd = T.readout(dev, prob)
+            r = T.check(prob, rd, lam, diag)
+            assert max(r.values()) <= 1.0, (model, f32, lam, r)
+            assert abs(e1 - T.linear_error(prob, rd)) <= 1e-9 * e0
+        dev.close()
+
+
 def coverage(_):
     """Kernel instantiations no fixture reaches (tests/emu/kernel_coverage.py): PriorFactor<Point3> outside the fused
     leaves (points ordered LAST, so their cliques are interior), Dogleg with FP32 Jacobian storage on every factor family
@@ -429,7 +454,7 @@ def coverage(_):
             os.environ.pop("B200_DF_ORDER"); os.environ.pop("B200_DF_LAG")
 
 
-SCEN = dict(coverage=coverage, midsize=midsize, edge=edge, bigfront=bigfront, gnc=gnc_scenario, typed=typed, fp32=fp32, linear=linear, marginals=marginals, dogleg=dogleg, gn=gn, mirror=linear_mirror)
+SCEN = dict(coverage=coverage, leafshapes=leafshapes, midsize=midsize, edge=edge, bigfront=bigfront, gnc=gnc_scenario, typed=typed, fp32=fp32, linear=linear, marginals=marginals, dogleg=dogleg, gn=gn, mirror=linear_mirror)
 for arg in sys.argv[2:]:
     kind, case = arg.split(":")
     t = time.time()

@@ -9,8 +9,9 @@ to 64 points (16 mini-batches, 4 per warp, a short last one where a camera set h
     go through the same per-point arithmetic; diagonal damping would bring in the Hessian diagonal, summed with atomics);
   * delta of a diagonally damped solve agrees with the split path to 1e-10 and with the oracle to 1e-8 (FP32 storage: 1e-5,
     the oracle rounds its own FP64 Jacobians to float, tests/test_gpu_precision.py);
-  * the LM error after two iterations agrees with the split path to 1e-10 and with the oracle to 1e-7 (FP32 storage: both
-    1e-5, the FP32 protocol of SURVEY 8(c)).
+  * the LM error after two iterations agrees with the split path to 1e-10 and with the oracle to 1e-7; with FP32 storage,
+    each LM iteration of either path agrees to 1e-5 (the FP32 protocol of SURVEY 8(c)) with an oracle iteration started
+    from the same values and lambda (two iterations in a row are chaotic there: see below).
 Own process; strict: any mismatch, crash or timeout fails with stderr."""
 import os
 import subprocess
@@ -74,19 +75,33 @@ for model, obs in (("cal3_s2", 5), ("cal3_s2", 6), ("bundler", 8)):
         errs = {{}}
         for mma, dev in devs.items():
             lm = optimizer.LevenbergMarquardtOptimizer(ctx, prob, device_problem=dev)
-            for _ in range(2):
-                lm.iterate()
-            errs[mma] = lm.error()
-            if mma == 1:
-                olm = orc.lm(lm.params()._c)
-                for _ in range(2):
+            if f32:
+                # FP32 storage: each path, iteration by iteration, against an oracle iteration from the same values and
+                # lambda.  Two iterations in a row are chaotic here: the atomics of the extend-add reorder sums, the barely
+                # damped (lambda = 1e-5) solve amplifies that, and the second linearization then rounds a different set of
+                # Jacobian entries to float.  The oracle alone, started from values 1e-10 apart, ends its second iteration
+                # up to 1.6e-4 apart (FP64 storage: 1.4e-10).
+                for it in range(2):
+                    orc.set_values(lm.values())
+                    olm = orc.lm(lm.params()._c)
+                    olm.state.lambda_ = lm.lambda_()
+                    lm.iterate()
                     orc.lm_iterate(olm)
-                assert abs(errs[1] - olm.state.error) <= (1e-5 if f32 else 1e-7) * olm.state.error, (model, obs, f32, errs[1], olm.state.error)
+                    print("fp32 LM", model, obs, "mma", mma, "iteration", it, "rel. diff %.3g" % (abs(lm.error() - olm.state.error) / olm.state.error))
+                    assert abs(lm.error() - olm.state.error) <= 1e-5 * olm.state.error, (model, obs, mma, it, lm.error(), olm.state.error)
+            else:
+                for _ in range(2):
+                    lm.iterate()
+                errs[mma] = lm.error()
+                if mma == 1:
+                    olm = orc.lm(lm.params()._c)
+                    for _ in range(2):
+                        orc.lm_iterate(olm)
+                    assert abs(errs[1] - olm.state.error) <= 1e-7 * olm.state.error, (model, obs, f32, errs[1], olm.state.error)
             del lm
             dev.close()
-        # (FP32 storage: two LM iterations of the same path already differ by up to ~1e-6 from run to run: the atomics of
-        # the extend-add reorder sums, and the second linearization rounds its Jacobians to float)
-        assert abs(errs[1] - errs[0]) <= (1e-5 if f32 else 1e-10) * errs[0], (model, obs, f32, errs)
+        if not f32:
+            assert abs(errs[1] - errs[0]) <= 1e-10 * errs[0], (model, obs, f32, errs)
         checked += len(conds[1])
 print("FUSED_OK", checked)
 """

@@ -44,6 +44,8 @@ GROUPS = [
     # ... and long runs of points per CTA (several cp.async batches, both batch sizes, 2 and 3 tiles per thread) in both storage modes
     # coverage: instantiations no fixture reaches (tests/emu/kernel_coverage.py lists what is left)
     ["edge:x", "coverage:x", "midsize:cal3_s2", "midsize:bundler", "midsize:bundler@8", "midsize:cal3_s2@8", "midsize:bundler@4", "midsize:cal3_s2@5", "midsize:bundler@3", "bigfront:x"],
+    # the BAL point leaves at mixed separator widths and run lengths (tests/test_point_leaf_shapes.py)
+    ["leafshapes:cal3_s2", "leafshapes:bundler"],
     # the GaussianFactorGraph level, Dogleg, Gauss-Newton
     ["linear:" + c for c in ("lin_pose2_toy", "lin_pose2_synth", "lin_random_nary", "lin_mixed_hessian", "lin_arity8", "lin_sphere_tiny",
                              "lin_bal_tiny", "lin_singular", "lin_family_sfm2", "lin_family_smart", "lin_family_expr")] +
