@@ -9,6 +9,7 @@
 #include <dlfcn.h>
 #include <cstring>
 #include <limits>
+#include <memory>
 #include <thread>
 
 #include "kernels.cuh"
@@ -48,13 +49,13 @@ static int noise_payload(int kind, int d) {
 }
 
 template <class T>
-static int upload(T** dst, const T* src, size_t n, cudaStream_t st) {
-  B200_CUDA(cudaMalloc((void**)dst, std::max<size_t>(n, 1) * sizeof(T)));
-  if (n) B200_CUDA(cudaMemcpyAsync(*dst, src, n * sizeof(T), cudaMemcpyHostToDevice, st));
-  return B200_OK;
+static cudaError_t upload(DevPtr<T>& dst, const T* src, size_t n, cudaStream_t st) {
+  cudaError_t e = dst.alloc(n);
+  if (e == cudaSuccess && n) e = cudaMemcpyAsync(dst, src, n * sizeof(T), cudaMemcpyHostToDevice, st);
+  return e;
 }
 template <class T>
-static int upload(T** dst, const std::vector<T>& v, cudaStream_t st) { return upload(dst, v.data(), v.size(), st); }
+static cudaError_t upload(DevPtr<T>& dst, const std::vector<T>& v, cudaStream_t st) { return upload(dst, v.data(), v.size(), st); }
 
 static GroupView view(const b200_problem::Group& g) {
   GroupView v;
@@ -262,14 +263,14 @@ static int enqueue_solve(b200_problem* p, bool damped, int diagonal, double min_
     // linearize, as the reference does, LevenbergMarquardtOptimizer.cpp:293-299), not once per lambda try
     if (diagonal && !p->hdiag_valid) { const int rc = enqueue_hdiag(p); if (rc) return rc; p->hdiag_valid = true; }
     launch_k(damp_kernel, dim3((int)((p->ndelta + 255) / 256)), dim3(256), 0, st, p->d_arena, p->d_diag_index, (int)p->ndelta, p->d_lambda,
-                                                                diagonal ? p->d_hdiag : nullptr, min_diag, max_diag);
+                                                                diagonal ? p->d_hdiag.get() : nullptr, min_diag, max_diag);
     ctx->launches++;
   }
   if (p->n_fused) {
     PhaseScope ps(p, PH_LEAF);
     GroupTable gt;
     for (size_t gi = 0; gi < p->groups.size(); gi++) gt.g[gi] = view(p->groups[gi]);
-    const double* hd = (damped && diagonal) ? p->d_hdiag : nullptr;
+    const double* hd = (damped && diagonal) ? p->d_hdiag.get() : nullptr;
     if (p->leaf_run_end[0] > p->leaf_run_begin[0]) {
       const int nr = p->leaf_run_end[0] - p->leaf_run_begin[0], nb = (nr + kWarpsPerBlock - 1) / kWarpsPerBlock;
       const size_t sm = (size_t)kWarpsPerBlock * p->leaf_lb_cap * sizeof(double);
@@ -359,7 +360,7 @@ static int enqueue_solve(b200_problem* p, bool damped, int diagonal, double min_
       v.tasks = tasks; v.ntasks = ntasks;
       v.ctrl = p->d_df_sync + 2 * slot; v.done = p->d_df_sync + p->df_ctrl_ints; v.flags = v.done + p->sym.ncliques;
       v.flag_off = p->d_df_flag_off; v.expect = p->d_df_expect;
-      v.trace = trace ? p->d_df_trace : nullptr;
+      v.trace = trace ? p->d_df_trace.get() : nullptr;
       v.winv = p->d_winv; v.winv_off = p->d_winv_off;
       v.warm_ctas = getenv("B200_DF_NO_WARM") ? 0 : 3 * ctx->sm_count;
       if (p->df_minb == 3) launch_k(front_df_kernel<3>, dim3(ntasks), dim3(kDfThreads), (size_t)kDfSmemBytes, st, t, v, p->d_scalars);
@@ -921,7 +922,7 @@ static int enqueue_try(b200_problem* p, int diagonal, double min_diag, double ma
   if (!rc) rc = enqueue_try_step(p);
   p->defer_scalar_reduce = false;
   if (rc || !merged) return rc;
-  if (!p->d_red) B200_CUDA(cudaMalloc((void**)&p->d_red, (3 + 2 * kMaxRanksMerged) * sizeof(double)));
+  if (!p->d_red) B200_CUDA(p->d_red.alloc(3 + 2 * kMaxRanksMerged));
   cudaStream_t st = p->ctx->stream;
   launch_k(scalars_pack_kernel, dim3(1), dim3(32), 0, st, p->d_scalars, p->d_red, p->ctx->rank, p->ctx->world, 0);
   rc = allreduce_sum(p, p->d_red, (size_t)(3 + 2 * p->ctx->world));
@@ -958,6 +959,11 @@ static int launch_try(b200_problem* p, int diagonal, double min_diag, double max
   p->solved = p->factored = true;
   p->marg_ready = false;     // the LM try factors the damped system
   return B200_OK;
+}
+// the captured LM tries have the group views, buffers and kernel instantiations baked in
+static void drop_try_graphs(b200_problem* p) {
+  for (auto& g : p->try_graph)
+    if (g) { cudaGraphExecDestroy(g); g = nullptr; }
 }
 
 }  // namespace b200
@@ -1007,6 +1013,14 @@ int b200_ctx_create(int device, b200_ctx** out) {
                                  (int)(kWarpsPerBlock * (kLeafMaxFN + kLeafAccMax) * sizeof(double))));
   B200_CUDA(cudaFuncSetAttribute(elim_small_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                  (int)(kWarpsPerBlock * kSmallMaxN * kSmallMaxN * sizeof(double))));
+  B200_CUDA(cudaFuncSetAttribute(front_df_kernel<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, kDfSmemBytes));
+  B200_CUDA(cudaFuncSetAttribute(front_df_kernel<3>, cudaFuncAttributeMaxDynamicSharedMemorySize, kDfSmemBytes));
+  // the widest point-leaf instantiations stage more than the 48 KB a kernel gets by default
+#define B200_SM_ATTR(DC_, T_)                                                                                                          \
+  B200_CUDA(cudaFuncSetAttribute(leaf_point_fused_mma_kernel<DC_, T_, double>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024)); \
+  B200_CUDA(cudaFuncSetAttribute(leaf_point_fused_mma_kernel<DC_, T_, float>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
+  B200_SM_ATTR(6, 4) B200_SM_ATTR(6, 5) B200_SM_ATTR(6, 7) B200_SM_ATTR(9, 4) B200_SM_ATTR(9, 5) B200_SM_ATTR(9, 7) B200_SM_ATTR(9, 10)
+#undef B200_SM_ATTR
 #endif
   guard.c = nullptr;
   *out = c;
@@ -1045,68 +1059,35 @@ int b200_problem_destroy(b200_problem* p) {
   if (!p) return B200_OK;
   cudaSetDevice(p->ctx->device);
   cudaStreamSynchronize(p->ctx->stream);
-  for (auto& g : p->groups) {
-    cudaFree(g.d_keys); cudaFree(g.d_meas); cudaFree(g.d_noise); cudaFree(g.d_cal); cudaFree(g.d_body); cudaFree(g.d_J); cudaFree(g.d_scat);
-    cudaFree(g.d_jkeys); cudaFree(g.d_jslots); cudaFree(g.d_jclique);
-  }
-  cudaFree(p->d_values); cudaFree(p->d_new_values); cudaFree(p->d_delta); cudaFree(p->d_hdiag); cudaFree(p->d_grad);
-  cudaFree(p->d_val_off); cudaFree(p->d_var_type); cudaFree(p->d_var_dof); cudaFree(p->d_cal); cudaFree(p->d_arena);
-  cudaFree(p->d_off); cudaFree(p->d_nf); cudaFree(p->d_ns); cudaFree(p->d_parent); cudaFree(p->d_ea_ptr);
-  cudaFree(p->d_didx_ptr); cudaFree(p->d_ea_map); cudaFree(p->d_didx); cudaFree(p->d_diag_index);
-  cudaFree(p->d_lvl_small); cudaFree(p->d_lvl_bsmall); cudaFree(p->d_lvl_blarge); cudaFree(p->d_marg_work); cudaFree(p->d_marg_path); cudaFree(p->d_marg_out); cudaFree(p->d_lvl_bpoint); cudaFree(p->d_ld);
-  cudaFree(p->d_bs_flags); cudaFree(p->d_bs_flag_base);
-  cudaFree(p->d_df_tasks[0]); cudaFree(p->d_df_tasks[1]); cudaFree(p->d_df_flag_off); cudaFree(p->d_df_expect); cudaFree(p->d_df_sync); cudaFree(p->d_df_trace);
-  cudaFree(p->d_winv); cudaFree(p->d_winv_off); cudaFree(p->d_red);
-  cudaFree(p->d_view_idx[0]); cudaFree(p->d_view_idx[1]); cudaFree(p->d_view_buf); cudaFree(p->d_gather_buf);
-  cudaFree(p->d_ts_cliques); cudaFree(p->d_ts_xoff); cudaFree(p->d_ts_owned); cudaFree(p->d_topx);
-  cudaFree(p->d_fused_run_ptr);
-  cudaFree(p->d_fused_list); cudaFree(p->d_fused_fac_ptr); cudaFree(p->d_fused_fac); cudaFree(p->d_pt_tab); cudaFree(p->d_pt_off); cudaFree(p->d_partials); cudaFree(p->d_counters); cudaFree(p->d_scalars);
-  cudaFreeHost(p->h_scalars); cudaFreeHost(p->h_pinned); cudaFreeHost(p->h_lambda); cudaFree(p->d_lambda);
-  for (int i = 0; i < 2; i++) if (p->try_graph[i]) cudaGraphExecDestroy(p->try_graph[i]);
-  cudaFree(p->d_saved_values);
+  drop_try_graphs(p);
   for (auto& e : p->ev_pool) { cudaEventDestroy(e.first); cudaEventDestroy(e.second); }
-  delete p;
+  delete p;   // the owners of the problem's buffers free them
   return B200_OK;
 }
-
 static int upload_jacobian_group(b200_problem* p, b200_problem::Group& g, const double* Ab, const double* sigmas);
 
-// Problem creation, shared by the two descriptions: `d` (nonlinear graph + Values, b200_problem_create) or
-// `ld` (JacobianFactors, b200_linear_create); exactly one of them is non-null.
-static int create_problem(b200_ctx* ctx, const b200_problem_desc* d, const b200_linear_desc* ld, b200_problem** out) {
-  if (!ctx || (!d && !ld) || !out) { set_error("null argument"); return B200_INVALID_ARGUMENT; }
-  B200_CUDA(cudaSetDevice(ctx->device));
-  cudaStream_t st = ctx->stream;
-  b200_problem* p = new b200_problem();
-  p->ctx = ctx;
-  p->linear = ld != nullptr;
-#define FAIL(code, msg) do { set_error(msg); b200_problem_destroy(p); return code; } while (0)
-  // B200_SETUP_TIMING=1: where the one-time setup goes (host wall clock per stage, stderr)
-  const bool setup_timing = getenv("B200_SETUP_TIMING") != nullptr;
-  auto t_prev = std::chrono::steady_clock::now();
-  auto lap = [&](const char* what) {
-    if (!setup_timing) return;
-    const auto now = std::chrono::steady_clock::now();
-    fprintf(stderr, "[b200 setup] %-28s %8.1f ms\n", what, std::chrono::duration<double, std::milli>(now - t_prev).count());
-    t_prev = now;
-  };
+// What the stages of create_problem hand on to each other.
+struct ProblemPlan {
+  const b200_problem_desc* d; const b200_linear_desc* ld;   // exactly one of them is non-null
+  int64_t ngroups = 0;
   Packed pk;
-  {
-    const int rc = d ? pack_and_symbolic(d, &pk) : pack_linear(ld, &pk);
-    if (rc) { b200_problem_destroy(p); return rc; }
-  }
-  lap("validate + symbolic phase");
-  const int64_t n = d ? d->nvars : ld->nvars;
-  const int64_t ngroups = d ? d->ngroups : ld->ngroups + ld->nhgroups;   // linear: Jacobian groups, then Hessian groups
-  const int64_t total = pk.total;
-  p->nvars = n; p->nval = pk.val_off[n]; p->ndelta = pk.var_dof[n]; p->nfactors = total;
-  if (d) p->var_type.assign(d->var_type, d->var_type + n);
-  std::vector<int>&val_off = pk.val_off, &var_dof = pk.var_dof, &var_dim = pk.var_dim;
-  std::vector<int64_t>&fptr = pk.fptr, &fkeys = pk.fkeys;
-  p->groups.resize(ngroups);
-  for (int64_t gi = 0; gi < ngroups; gi++) {
+  std::vector<char> fused, is_top;                          // per clique (shard_plan)
+  std::vector<int> clique_owner, factor_owner, top_owner;
+  std::vector<int> fused_list, run_ptr;                     // the fused leaf cliques THIS rank owns, in runs
+  std::vector<int> leaf_kind;                               // per clique: 0 generic, 1 / 2: BAL point clique, 6- / 9-dof cameras
+  std::vector<std::vector<int2>> hkeys; std::vector<std::vector<int4>> hscat;   // typed groups: keys, scatter records (device order)
+};
+
+static int setup_symbolic(b200_problem* p, ProblemPlan& P) {
+  if (const int rc = P.d ? pack_and_symbolic(P.d, &P.pk) : pack_linear(P.ld, &P.pk)) return rc;
+  const int64_t n = P.d ? P.d->nvars : P.ld->nvars;
+  P.ngroups = P.d ? P.d->ngroups : P.ld->ngroups + P.ld->nhgroups;   // linear: Jacobian groups, then Hessian groups
+  p->nvars = n; p->nval = P.pk.val_off[n]; p->ndelta = P.pk.var_dof[n]; p->nfactors = P.pk.total;
+  if (P.d) p->var_type.assign(P.d->var_type, P.d->var_type + n);
+  p->groups.resize(P.ngroups);
+  for (int64_t gi = 0; gi < P.ngroups; gi++) {
     auto& g = p->groups[gi];
-    const PackedGroup& q = pk.groups[gi];
+    const PackedGroup& q = P.pk.groups[gi];
     g.type = q.type; g.noise_kind = q.noise_kind; g.per_factor = q.per_factor; g.noise_size = q.noise_size;
     g.d = q.d; g.ncols = q.ncols; g.arity = q.arity; g.meas = q.meas; g.count = q.count; g.pos = q.pos;
     g.robust_kind = q.robust_kind; g.robust_param = q.robust_param;
@@ -1114,168 +1095,141 @@ static int create_problem(b200_ctx* ctx, const b200_problem_desc* d, const b200_
     for (int a = 0; a < B200_JACOBIAN_MAX_ARITY; a++) g.col0[a + 1] = g.col0[a] + (a < q.arity ? q.dims[a] : 0);
     g.col0[q.arity + 1] = g.col0[q.arity] + 1;   // the rhs column closes the list
   }
-  p->sym = std::move(pk.sym);
+  p->sym = std::move(P.pk.sym);
+  return B200_OK;
+}
+static int setup_values(b200_problem* p, ProblemPlan& P) {
+  if (P.d) {
+    B200_CUDA(upload(p->d_values, P.d->values, (size_t)p->nval, p->ctx->stream));
+    B200_CUDA(p->d_new_values.alloc(p->nval));
+    B200_CUDA(upload(p->d_val_off, P.pk.val_off, p->ctx->stream));
+    B200_CUDA(upload(p->d_var_type, p->var_type, p->ctx->stream));
+    B200_CUDA(upload(p->d_cal, P.d->cal, (size_t)P.d->ncal * 5, p->ctx->stream));
+  }
+  B200_CUDA(p->d_delta.alloc(p->ndelta));
+  B200_CUDA(cudaMemsetAsync(p->d_delta, 0, std::max<int64_t>(1, p->ndelta) * sizeof(double), p->ctx->stream));
+  B200_CUDA(p->d_hdiag.alloc(p->ndelta));
+  B200_CUDA(upload(p->d_var_dof, P.pk.var_dof, p->ctx->stream));
+  return B200_OK;
+}
+// Storage plan (fused leaf cliques keep only their f x n conditional; sharding), then the owned fused leaves grouped into
+// runs that share (parent, separator variables): one warp / CTA reduces a run's Schur complements before the extend-add.
+static int setup_leaf_runs(b200_problem* p, ProblemPlan& P) {
   const Symbolic& S = p->sym;
-#define UP(call) do { int rc_ = (call); if (rc_) { b200_problem_destroy(p); return rc_; } } while (0)
-  // ---- values & variable tables ----
-  if (d) {
-    UP(upload(&p->d_values, d->values, (size_t)p->nval, st));
-    B200_CUDA(cudaMalloc((void**)&p->d_new_values, std::max<int64_t>(1, p->nval) * sizeof(double)));
-    UP(upload(&p->d_val_off, val_off, st));
-    UP(upload(&p->d_var_type, p->var_type, st));
-    UP(upload(&p->d_cal, d->cal, (size_t)d->ncal * 5, st));
-  }
-  B200_CUDA(cudaMalloc((void**)&p->d_delta, std::max<int64_t>(1, p->ndelta) * sizeof(double)));
-  B200_CUDA(cudaMemsetAsync(p->d_delta, 0, std::max<int64_t>(1, p->ndelta) * sizeof(double), st));
-  B200_CUDA(cudaMalloc((void**)&p->d_hdiag, std::max<int64_t>(1, p->ndelta) * sizeof(double)));
-  UP(upload(&p->d_var_dof, var_dof, st));
-  lap("values + variable tables");
-  // ---- storage plan: fused leaf cliques keep only their f x n conditional; sharding -----
-  std::vector<char> fused, is_top;
-  std::vector<int> clique_owner, factor_owner, top_owner;
-  shard_plan(S, ngroups, total, ctx->world, &fused, &is_top, &clique_owner, &factor_owner, /*allow_leaf=*/d != nullptr, &top_owner);
-  const int rank = ctx->rank;
+  const b200_ctx* ctx = p->ctx;
+  shard_plan(S, P.ngroups, p->nfactors, ctx->world, &P.fused, &P.is_top, &P.clique_owner, &P.factor_owner, /*allow_leaf=*/P.d != nullptr, &P.top_owner);
   p->top_staged = ctx->world > 1 && getenv("B200_REPLICATED_TOP") == nullptr;
-  std::vector<int> fused_list;   // the fused leaf cliques THIS rank owns
+  std::vector<int>& fused_list = P.fused_list;
   for (int64_t c = 0; c < S.ncliques; c++)
-    if (fused[c] && clique_owner[c] == rank) fused_list.push_back((int)c);
-  // group the owned fused leaves into runs that share (parent, separator variables): one warp
-  // reduces a run's Schur complements in shared memory before the extend-add
-  std::vector<int> run_ptr;
-  std::vector<int> leaf_kind(S.ncliques, 0);   // 0 generic, 1 / 2: BAL point clique with 6- / 9-dof cameras
-  {
-    auto sig_less = [&](int a, int b) {
-      if (S.parent[a] != S.parent[b]) return S.parent[a] < S.parent[b];
-      const int64_t la = S.sep_ptr[a + 1] - S.sep_ptr[a], lb = S.sep_ptr[b + 1] - S.sep_ptr[b];
-      if (la != lb) return la < lb;
-      for (int64_t q = 0; q < la; q++) {
-        const int64_t va = S.sep_vars[S.sep_ptr[a] + q], vb = S.sep_vars[S.sep_ptr[b] + q];
-        if (va != vb) return va < vb;
-      }
-      return a < b;
-    };
-    auto sig_eq = [&](int a, int b) {
-      if (S.parent[a] != S.parent[b] || S.ns[a] != S.ns[b]) return false;
-      const int64_t la = S.sep_ptr[a + 1] - S.sep_ptr[a];
-      if (la != S.sep_ptr[b + 1] - S.sep_ptr[b]) return false;
-      for (int64_t q = 0; q < la; q++)
-        if (S.sep_vars[S.sep_ptr[a] + q] != S.sep_vars[S.sep_ptr[b] + q]) return false;
-      return true;
-    };
-    // kind 1/2: BAL point cliques (one Point3 frontal, m <= kPtMaxObs binary projection factors on
-    // distinct cameras) take leaf_point_{factor,schur}_kernel<6>/<9>; everything else the generic leaf kernel
-    std::vector<int> cf_count(S.ncliques, 0), cf_mask(S.ncliques, 0);
-    std::vector<int>& kind = leaf_kind;
-    for (int64_t gi = 0; d && gi < d->ngroups; gi++)
-      for (int64_t i = 0; i < d->groups[gi].count; i++) {
-        const int c = S.fac_clique[p->groups[gi].pos[i]];
-        if (fused[c]) { cf_count[c]++; cf_mask[c] |= 1 << d->groups[gi].type; }
-      }
-    const bool fast = !getenv("B200_NO_POINT_KERNEL");
-    for (int c : fused_list) {
-      const int64_t nsep = S.sep_ptr[c + 1] - S.sep_ptr[c];
-      const bool point = S.front_ptr[c + 1] - S.front_ptr[c] == 1 && d->var_type[S.front_vars[S.front_ptr[c]]] == B200_VAR_POINT3;
-      if (!fast || !point || cf_count[c] != nsep || cf_count[c] > kPtMaxObs || cf_count[c] < 1) continue;
-      if (cf_mask[c] == (1 << B200_FACTOR_PROJECTION_CAL3S2)) kind[c] = 1;
-      else if (cf_mask[c] == (1 << B200_FACTOR_SFM_BUNDLER)) kind[c] = 2;
+    if (P.fused[c] && P.clique_owner[c] == p->ctx->rank) fused_list.push_back((int)c);
+  auto sig_cmp = [&](int a, int b) {   // run signature: parent, then the separator variables
+    if (S.parent[a] != S.parent[b]) return S.parent[a] < S.parent[b] ? -1 : 1;
+    const int64_t la = S.sep_ptr[a + 1] - S.sep_ptr[a], lb = S.sep_ptr[b + 1] - S.sep_ptr[b];
+    if (la != lb) return la < lb ? -1 : 1;
+    for (int64_t q = 0; q < la; q++) {
+      const int64_t va = S.sep_vars[S.sep_ptr[a] + q], vb = S.sep_vars[S.sep_ptr[b] + q];
+      if (va != vb) return va < vb ? -1 : 1;
     }
-    std::sort(fused_list.begin(), fused_list.end(), [&](int a, int b) {
-      if (kind[a] != kind[b]) return kind[a] < kind[b];
-      return sig_less(a, b);
-    });
-    const int nfl = (int)fused_list.size();
-    // long enough to amortise the per-run extend-add, short enough for >= 8 CTAs per SM
-    int run_max_pt = getenv("B200_NO_LEAF_RUNS") ? 1 : std::max(1, std::min(64, nfl / (ctx->sm_count * 8)));
-    if (getenv("B200_LEAF_RUN_MAX")) run_max_pt = std::max(1, atoi(getenv("B200_LEAF_RUN_MAX")));
-    run_ptr.push_back(0);
-    for (int kd = 0; kd < 3; kd++) p->leaf_run_begin[kd] = p->leaf_run_end[kd] = 0;
-    for (int i = 1; i <= nfl; i++) {
-      const int kprev = kind[fused_list[i - 1]];
-      const int rmax = kprev == 0 ? 1 : run_max_pt;
-      if (i == nfl || i - run_ptr.back() >= rmax || kind[fused_list[i]] != kprev || !sig_eq(fused_list[i - 1], fused_list[i])) {
-        run_ptr.push_back(i);
-      }
+    return 0;
+  };
+  // kind 1/2: BAL point cliques (one Point3 frontal, m <= kPtMaxObs binary projection factors on
+  // distinct cameras) take the point-leaf kernels <6>/<9>; everything else the generic leaf kernel
+  std::vector<int> cf_count(S.ncliques, 0), cf_mask(S.ncliques, 0);
+  std::vector<int>& kind = P.leaf_kind;
+  kind.assign(S.ncliques, 0);
+  for (int64_t gi = 0; P.d && gi < P.d->ngroups; gi++)
+    for (int64_t i = 0; i < P.d->groups[gi].count; i++) {
+      const int c = S.fac_clique[p->groups[gi].pos[i]];
+      if (P.fused[c]) { cf_count[c]++; cf_mask[c] |= 1 << P.d->groups[gi].type; }
     }
-    p->n_runs = (int)run_ptr.size() - 1;
-    {
-      int r = 0;
-      for (int kd = 0; kd < 3; kd++) {
-        p->leaf_run_begin[kd] = r;
-        while (r < p->n_runs && kind[fused_list[run_ptr[r]]] == kd) r++;
-        p->leaf_run_end[kd] = r;
-        p->leaf_pos_begin[kd] = run_ptr[p->leaf_run_begin[kd]];
-        p->leaf_pos_end[kd] = run_ptr[r];
-      }
-    }
-    // shared memory per warp: the widest [F S d] block (generic) / packed Schur triangle (point kernels)
-    int lb = 1, tri = 0;
-    for (int c : fused_list) {
-      const int nn = S.nf[c] + S.ns[c] + 1, w = S.ns[c] + 1;
-      if (kind[c] == 0) lb = std::max(lb, S.nf[c] * nn);
-    }
-    p->leaf_lb_cap = lb; p->leaf_acc_cap = tri;
-    for (int c : fused_list) p->leaf_max_w[kind[c]] = std::max(p->leaf_max_w[kind[c]], S.ns[c] + 1);
+  const bool fast = !getenv("B200_NO_POINT_KERNEL");
+  for (int c : fused_list) {
+    const int64_t nsep = S.sep_ptr[c + 1] - S.sep_ptr[c];
+    const bool point = S.front_ptr[c + 1] - S.front_ptr[c] == 1 && P.d->var_type[S.front_vars[S.front_ptr[c]]] == B200_VAR_POINT3;
+    if (!fast || !point || cf_count[c] != nsep || cf_count[c] > kPtMaxObs || cf_count[c] < 1) continue;
+    if (cf_mask[c] == (1 << B200_FACTOR_PROJECTION_CAL3S2)) kind[c] = 1;
+    else if (cf_mask[c] == (1 << B200_FACTOR_SFM_BUNDLER)) kind[c] = 2;
   }
-  lap("shard plan + leaf runs");
-  p->n_fused = (int)fused_list.size();
+  std::sort(fused_list.begin(), fused_list.end(), [&](int a, int b) {
+    if (kind[a] != kind[b]) return kind[a] < kind[b];
+    const int s = sig_cmp(a, b);
+    return s != 0 ? s < 0 : a < b;
+  });
+  const int nfl = (int)fused_list.size();
+  // long enough to amortise the per-run extend-add, short enough for >= 8 CTAs per SM
+  int run_max_pt = getenv("B200_NO_LEAF_RUNS") ? 1 : std::max(1, std::min(64, nfl / (ctx->sm_count * 8)));
+  if (getenv("B200_LEAF_RUN_MAX")) run_max_pt = std::max(1, atoi(getenv("B200_LEAF_RUN_MAX")));
+  std::vector<int>& run_ptr = P.run_ptr;
+  run_ptr.push_back(0);
+  for (int i = 1; i <= nfl; i++) {
+    const int kprev = kind[fused_list[i - 1]];
+    const int rmax = kprev == 0 ? 1 : run_max_pt;
+    if (i == nfl || i - run_ptr.back() >= rmax || kind[fused_list[i]] != kprev || sig_cmp(fused_list[i - 1], fused_list[i]) != 0)
+      run_ptr.push_back(i);
+  }
+  p->n_runs = (int)run_ptr.size() - 1;
+  for (int kd = 0, r = 0; kd < 3; kd++) {
+    p->leaf_run_begin[kd] = r;
+    while (r < p->n_runs && kind[fused_list[run_ptr[r]]] == kd) r++;
+    p->leaf_run_end[kd] = r;
+    p->leaf_pos_begin[kd] = run_ptr[p->leaf_run_begin[kd]];
+    p->leaf_pos_end[kd] = run_ptr[r];
+  }
+  // shared memory per warp of the generic leaf kernel: the widest [F S d] block
+  for (int c : fused_list) {
+    if (kind[c] == 0) p->leaf_lb_cap = std::max(p->leaf_lb_cap, S.nf[c] * (S.nf[c] + S.ns[c] + 1));
+    p->leaf_max_w[kind[c]] = std::max(p->leaf_max_w[kind[c]], S.ns[c] + 1);
+  }
+  p->n_fused = nfl;
   p->schur_pb = (getenv("B200_SCHUR_PB") && atoi(getenv("B200_SCHUR_PB")) == 6) ? 6 : 4;
   p->schur_mma = !(getenv("B200_SCHUR_MMA") && atoi(getenv("B200_SCHUR_MMA")) == 0);
   if (getenv("B200_LIN_VARIANT")) p->lin_variant = atoi(getenv("B200_LIN_VARIANT"));
-#ifndef B200_EMULATE
-  {   // the widest instantiations stage more than the 48 KB a kernel gets by default
-    const int optin = 200 * 1024;
-#define B200_SM_ATTR(DC_, T_)                                                                                                          \
-    B200_CUDA(cudaFuncSetAttribute(leaf_point_fused_mma_kernel<DC_, T_, double>, cudaFuncAttributeMaxDynamicSharedMemorySize, optin)); \
-    B200_CUDA(cudaFuncSetAttribute(leaf_point_fused_mma_kernel<DC_, T_, float>, cudaFuncAttributeMaxDynamicSharedMemorySize, optin));
-    B200_SM_ATTR(6, 4) B200_SM_ATTR(6, 5) B200_SM_ATTR(6, 7) B200_SM_ATTR(9, 4) B200_SM_ATTR(9, 5) B200_SM_ATTR(9, 7) B200_SM_ATTR(9, 10)
-#undef B200_SM_ATTR
-  }
-#endif
+  return B200_OK;
+}
+static int setup_offsets(b200_problem* p, ProblemPlan& P) {
+  const Symbolic& S = p->sym;
   p->h_off.assign(S.ncliques + 1, 0);
   p->h_ld.assign(S.ncliques, 0);
-  {
-    int64_t o = 0;
-    std::vector<int64_t> order(S.ncliques);     // top fronts level by level: a stage of the distributed top is one contiguous range
-    for (int64_t c = 0; c < S.ncliques; c++) order[c] = c;
-    std::stable_sort(order.begin(), order.end(), [&](int64_t a, int64_t b) { return (is_top[a] ? S.level[a] : -1) < (is_top[b] ? S.level[b] : -1); });
-    for (int pass = 0; pass < 2; pass++) {   // replicated top first: it is the all-reduced region
-      for (int64_t oc = 0; oc < S.ncliques; oc++) {
-        const int64_t c = pass == 0 ? order[oc] : oc;
-        if (!fused[c] && (is_top[c] != 0) == (pass == 0)) {
-          const int64_t nn = S.nf[c] + S.ns[c] + 1; p->h_ld[c] = (int)nn;
-          // the fronts of other ranks' subtrees take no storage here (nothing on this rank ever touches them)
-          if (pass == 1 && clique_owner[c] != rank) { p->h_off[c] = 0; continue; }
-          p->h_off[c] = o; o += nn * nn;
-        }
+  int64_t o = 0;
+  std::vector<int64_t> order(S.ncliques);     // top fronts level by level: a stage of the distributed top is one contiguous range
+  for (int64_t c = 0; c < S.ncliques; c++) order[c] = c;
+  std::stable_sort(order.begin(), order.end(), [&](int64_t a, int64_t b) { return (P.is_top[a] ? S.level[a] : -1) < (P.is_top[b] ? S.level[b] : -1); });
+  for (int pass = 0; pass < 2; pass++) {   // replicated top first: it is the all-reduced region
+    for (int64_t oc = 0; oc < S.ncliques; oc++) {
+      const int64_t c = pass == 0 ? order[oc] : oc;
+      if (!P.fused[c] && (P.is_top[c] != 0) == (pass == 0)) {
+        const int64_t nn = S.nf[c] + S.ns[c] + 1; p->h_ld[c] = (int)nn;
+        // the fronts of other ranks' subtrees take no storage here (nothing on this rank ever touches them)
+        if (pass == 1 && P.clique_owner[c] != p->ctx->rank) { p->h_off[c] = 0; continue; }
+        p->h_off[c] = o; o += nn * nn;
       }
-      if (pass == 0) p->top_doubles = o;
     }
-    p->zero_doubles = o;   // everything below is accumulated into by atomics: zeroed per solve
-    for (int64_t c = 0; c < S.ncliques; c++)
-      if (fused[c]) {
-        const int64_t nn = S.nf[c] + S.ns[c] + 1; p->h_ld[c] = S.nf[c];
-        if (clique_owner[c] != rank) { p->h_off[c] = 0; continue; }
-        p->h_off[c] = o; o += (int64_t)S.nf[c] * nn;
-      }
-    p->arena_doubles = o;
-    p->h_off[S.ncliques] = o;
+    if (pass == 0) p->top_doubles = o;
   }
-  lap("front offsets");
-  // ---- factor tables ----
-  const bool reorder_leaf_factors = getenv("B200_NO_FACTOR_REORDER") == nullptr;
-  std::vector<int> leaf_list_pos(S.ncliques, INT_MAX);      // position of a point leaf (kinds 1 / 2) in fused_list
-  for (size_t i = 0; i < fused_list.size(); i++) if (leaf_kind[fused_list[i]] > 0) leaf_list_pos[fused_list[i]] = (int)i;
-  std::vector<std::vector<int2>> hkeys(ngroups);
-  std::vector<std::vector<int4>> hscat(ngroups);
-  for (int64_t gi = 0; ld && gi < ngroups; gi++) {
-    // JacobianFactor / HessianFactor groups: keys, owning clique and front slot of every key, then the numbers
-    // (whitened [A|b], or the augmented information matrix) in the element-major SoA
+  p->zero_doubles = o;   // everything below is accumulated into by atomics: zeroed per solve
+  for (int64_t c = 0; c < S.ncliques; c++)
+    if (P.fused[c]) {
+      const int64_t nn = S.nf[c] + S.ns[c] + 1; p->h_ld[c] = S.nf[c];
+      if (P.clique_owner[c] != p->ctx->rank) { p->h_off[c] = 0; continue; }
+      p->h_off[c] = o; o += (int64_t)S.nf[c] * nn;
+    }
+  p->arena_doubles = o;
+  p->h_off[S.ncliques] = o;
+  return B200_OK;
+}
+// JacobianFactor / HessianFactor groups: keys, owning clique and front slot of every key, then the numbers
+// (whitened [A|b], or the augmented information matrix) in the element-major SoA
+static int setup_linear_groups(b200_problem* p, ProblemPlan& P) {
+  if (!P.ld) return B200_OK;
+  const Symbolic& S = p->sym;
+  const b200_linear_desc* ld = P.ld;
+  for (int64_t gi = 0; gi < P.ngroups; gi++) {
     auto& g = p->groups[gi];
     const bool hess = gi >= ld->ngroups;
     const int ar = g.arity;
-    // keep only the factors this rank owns (all of them when world == 1): SURVEY 8(e), as for the typed groups below
+    // keep only the factors this rank owns (all of them when world == 1): SURVEY 8(e), as for the typed groups
     g.full_count = g.count;
-    for (int64_t i = 0; i < g.full_count; i++) if (factor_owner[g.pos[i]] == rank) g.local_index.push_back(i);
+    for (int64_t i = 0; i < g.full_count; i++) if (P.factor_owner[g.pos[i]] == p->ctx->rank) g.local_index.push_back(i);
     const int64_t count = (int64_t)g.local_index.size();
     g.count = count;
     std::vector<int> jkeys((size_t)count * ar), jslots((size_t)count * ar), jclique((size_t)count);
@@ -1283,24 +1237,36 @@ static int create_problem(b200_ctx* ctx, const b200_problem_desc* d, const b200_
       const int64_t pos = g.pos[g.local_index[li]];
       jclique[li] = S.fac_clique[pos];
       for (int a = 0; a < ar; a++) {
-        jkeys[(size_t)li * ar + a] = (int)fkeys[fptr[pos] + a];
-        jslots[(size_t)li * ar + a] = S.fac_slots[fptr[pos] + a];
+        jkeys[(size_t)li * ar + a] = (int)P.pk.fkeys[P.pk.fptr[pos] + a];
+        jslots[(size_t)li * ar + a] = S.fac_slots[P.pk.fptr[pos] + a];
       }
     }
     g.n_nonleaf = count;
-    UP(upload(&g.d_jkeys, jkeys, st));
-    UP(upload(&g.d_jslots, jslots, st));
-    UP(upload(&g.d_jclique, jclique, st));
-    B200_CUDA(cudaMalloc((void**)&g.d_J, std::max<size_t>(1, (size_t)count * g.d * g.ncols) * sizeof(double)));
-    if (hess) UP(upload_jacobian_group(p, g, ld->hgroups[gi - ld->ngroups].info, nullptr));   // (N+1)^2 entries, no whitening
-    else UP(upload_jacobian_group(p, g, ld->groups[gi].Ab, ld->groups[gi].sigmas));
+    B200_CUDA(upload(g.d_jkeys, jkeys, p->ctx->stream));
+    B200_CUDA(upload(g.d_jslots, jslots, p->ctx->stream));
+    B200_CUDA(upload(g.d_jclique, jclique, p->ctx->stream));
+    B200_CUDA(g.d_J.alloc((size_t)count * g.d * g.ncols));
+    const int rc = hess ? upload_jacobian_group(p, g, ld->hgroups[gi - ld->ngroups].info, nullptr)   // (N+1)^2 entries, no whitening
+                        : upload_jacobian_group(p, g, ld->groups[gi].Ab, ld->groups[gi].sigmas);
+    if (rc) return rc;
   }
-  for (int64_t gi = 0; d && gi < ngroups; gi++) {
-    const b200_factor_group& s = d->groups[gi];
+  return B200_OK;
+}
+static int setup_typed_groups(b200_problem* p, ProblemPlan& P) {
+  if (!P.d) return B200_OK;
+  const Symbolic& S = p->sym;
+  const std::vector<int>& fused_list = P.fused_list;
+  const bool reorder_leaf_factors = getenv("B200_NO_FACTOR_REORDER") == nullptr;
+  std::vector<int> leaf_list_pos(S.ncliques, INT_MAX);      // position of a point leaf (kinds 1 / 2) in fused_list
+  for (size_t i = 0; i < fused_list.size(); i++) if (P.leaf_kind[fused_list[i]] > 0) leaf_list_pos[fused_list[i]] = (int)i;
+  P.hkeys.resize(P.ngroups);
+  P.hscat.resize(P.ngroups);
+  for (int64_t gi = 0; gi < P.ngroups; gi++) {
+    const b200_factor_group& s = P.d->groups[gi];
     auto& g = p->groups[gi];
     // keep only the factors this rank owns (all of them when world == 1)
     std::vector<int64_t>& keep = g.local_index;
-    for (int64_t i = 0; i < s.count; i++) if (factor_owner[g.pos[i]] == rank) keep.push_back(i);
+    for (int64_t i = 0; i < s.count; i++) if (P.factor_owner[g.pos[i]] == p->ctx->rank) keep.push_back(i);
     // Device order of a projection group = the order in which the leaf kernels visit its factors: by the position of the owning
     // point leaf in fused_list (points of one run next to each other), graph order inside a point; factors of other cliques
     // behind them.  Every row of the element-major SoA then holds a warp's 4 points x m factors contiguously.  In graph order
@@ -1320,8 +1286,9 @@ static int create_problem(b200_ctx* ctx, const b200_problem_desc* d, const b200_
       keep.swap(sorted);
     }
     const int64_t nl = (int64_t)keep.size();
-    hkeys[gi].resize(nl);
-    hscat[gi].resize(nl);
+    std::vector<int2>& hkeys = P.hkeys[gi];
+    std::vector<int4>& hscat = P.hscat[gi];
+    hkeys.resize(nl); hscat.resize(nl);
     std::vector<double> hmeas((size_t)nl * g.meas), hnoise;
     std::vector<int> hcal;
     if (s.noise_per_factor) hnoise.resize((size_t)nl * g.noise_size);
@@ -1331,10 +1298,10 @@ static int create_problem(b200_ctx* ctx, const b200_problem_desc* d, const b200_
     parallel_chunks(nl, [&](int64_t l0, int64_t l1, int tid) {
       int64_t nonleaf = 0;
       for (int64_t li = l0; li < l1; li++) {
-        const int64_t i = keep[li], pos = g.pos[i];
-        hkeys[gi][li] = make_int2((int)fkeys[fptr[pos]], g.arity == 2 ? (int)fkeys[fptr[pos] + 1] : -1);
-        const int isleaf = fused[S.fac_clique[pos]];
-        hscat[gi][li] = make_int4(S.fac_clique[pos], S.fac_slot0[pos], S.fac_slot1[pos], isleaf);
+        const int64_t i = keep[li], pos = g.pos[i], k0 = P.pk.fptr[pos];
+        hkeys[li] = make_int2((int)P.pk.fkeys[k0], g.arity == 2 ? (int)P.pk.fkeys[k0 + 1] : -1);
+        const int isleaf = P.fused[S.fac_clique[pos]];
+        hscat[li] = make_int4(S.fac_clique[pos], S.fac_slot0[pos], S.fac_slot1[pos], isleaf);
         if (!isleaf) nonleaf++;
         memcpy(hmeas.data() + (size_t)li * g.meas, s.meas + (size_t)i * g.meas, (size_t)g.meas * sizeof(double));
         if (s.noise_per_factor) memcpy(hnoise.data() + (size_t)li * g.noise_size, s.noise + (size_t)i * g.noise_size, (size_t)g.noise_size * sizeof(double));
@@ -1344,157 +1311,208 @@ static int create_problem(b200_ctx* ctx, const b200_problem_desc* d, const b200_
     });
     for (int t = 0; t < 16; t++) g.n_nonleaf += nonleaf_part[t];
     g.count = nl;
-    UP(upload(&g.d_keys, hkeys[gi], st));
-    UP(upload(&g.d_scat, hscat[gi], st));
-    UP(upload(&g.d_meas, hmeas, st));
-    if (s.noise_per_factor) UP(upload(&g.d_noise, hnoise, st));
-    else UP(upload(&g.d_noise, s.noise, (size_t)g.noise_size, st));
-    if (!hcal.empty()) UP(upload(&g.d_cal, hcal, st));
-    if (s.type == B200_FACTOR_PROJECTION_CAL3S2 && s.body_P_sensor) UP(upload(&g.d_body, s.body_P_sensor, 12, st));
-    B200_CUDA(cudaMalloc((void**)&g.d_J, std::max<size_t>(1, (size_t)nl * g.d * g.ncols) * sizeof(double)));
+    B200_CUDA(upload(g.d_keys, hkeys, p->ctx->stream));
+    B200_CUDA(upload(g.d_scat, hscat, p->ctx->stream));
+    B200_CUDA(upload(g.d_meas, hmeas, p->ctx->stream));
+    if (s.noise_per_factor) B200_CUDA(upload(g.d_noise, hnoise, p->ctx->stream));
+    else B200_CUDA(upload(g.d_noise, s.noise, (size_t)g.noise_size, p->ctx->stream));
+    if (!hcal.empty()) B200_CUDA(upload(g.d_cal, hcal, p->ctx->stream));
+    if (s.type == B200_FACTOR_PROJECTION_CAL3S2 && s.body_P_sensor) B200_CUDA(upload(g.d_body, s.body_P_sensor, 12, p->ctx->stream));
+    B200_CUDA(g.d_J.alloc((size_t)nl * g.d * g.ncols));
   }
-  lap("factor tables");
-  // ---- junction tree tables ----
+  return B200_OK;
+}
+static int setup_tree_tables(b200_problem* p, ProblemPlan& P) {
+  const Symbolic& S = p->sym;
   std::vector<int> parent32(S.ncliques);
   for (int64_t c = 0; c < S.ncliques; c++) parent32[c] = (int)S.parent[c];
-  UP(upload(&p->d_off, p->h_off, st));
-  UP(upload(&p->d_ld, p->h_ld, st));
-  UP(upload(&p->d_nf, S.nf, st));
-  UP(upload(&p->d_ns, S.ns, st));
-  UP(upload(&p->d_parent, parent32, st));
-  UP(upload(&p->d_ea_ptr, S.ea_ptr, st));
-  UP(upload(&p->d_ea_map, S.ea_map, st));
-  UP(upload(&p->d_didx_ptr, S.didx_ptr, st));
-  UP(upload(&p->d_didx, S.didx, st));
+  B200_CUDA(upload(p->d_off, p->h_off, p->ctx->stream));
+  B200_CUDA(upload(p->d_ld, p->h_ld, p->ctx->stream));
+  B200_CUDA(upload(p->d_nf, S.nf, p->ctx->stream));
+  B200_CUDA(upload(p->d_ns, S.ns, p->ctx->stream));
+  B200_CUDA(upload(p->d_parent, parent32, p->ctx->stream));
+  B200_CUDA(upload(p->d_ea_ptr, S.ea_ptr, p->ctx->stream));
+  B200_CUDA(upload(p->d_ea_map, S.ea_map, p->ctx->stream));
+  B200_CUDA(upload(p->d_didx_ptr, S.didx_ptr, p->ctx->stream));
+  B200_CUDA(upload(p->d_didx, S.didx, p->ctx->stream));
   std::vector<int64_t> diag_index(p->ndelta);
-  for (int64_t v = 0; v < n; v++) {
+  for (int64_t v = 0; v < p->nvars; v++) {
     const int c = S.var_clique[v];
     const int64_t nn = S.nf[c] + S.ns[c] + 1;
-    for (int k = 0; k < var_dim[v]; k++)
-      diag_index[var_dof[v] + k] = (fused[c] || (is_top[c] ? rank != 0 : clique_owner[c] != rank))
-                                       ? -1 : p->h_off[c] + (S.var_slot[v] + k) * (nn + 1);
+    for (int k = 0; k < P.pk.var_dim[v]; k++)
+      diag_index[P.pk.var_dof[v] + k] = (P.fused[c] || (P.is_top[c] ? p->ctx->rank != 0 : P.clique_owner[c] != p->ctx->rank))
+                                            ? -1 : p->h_off[c] + (S.var_slot[v] + k) * (nn + 1);
   }
-  UP(upload(&p->d_diag_index, diag_index, st));
-  lap("tree tables");
-  // fused leaf cliques: CSR of their factors as (group, index), graph order
-  if (p->n_fused) {
-    std::vector<int> lpos(S.ncliques, -1), fptr(p->n_fused + 1, 0);
-    for (int i = 0; i < p->n_fused; i++) lpos[fused_list[i]] = i;
-    for (int64_t pos = 0; pos < total; pos++) if (lpos[S.fac_clique[pos]] >= 0) fptr[lpos[S.fac_clique[pos]] + 1]++;
-    for (int i = 0; i < p->n_fused; i++) fptr[i + 1] += fptr[i];
-    std::vector<int2> ffac(fptr[p->n_fused]);
-    std::vector<int> cur(fptr.begin(), fptr.end() - 1);
-    for (int64_t gi = 0; gi < ngroups; gi++)
-      for (int64_t li = 0; li < p->groups[gi].count; li++) {
-        const int64_t pos = p->groups[gi].pos[p->groups[gi].local_index[li]];
-        if (lpos[S.fac_clique[pos]] >= 0) ffac[cur[lpos[S.fac_clique[pos]]]++] = make_int2((int)gi, (int)li);
-      }
-    // keep graph order inside each clique (groups may interleave in the graph; a clique whose factors come from one group
-    // already has it)
+  B200_CUDA(upload(p->d_diag_index, diag_index, p->ctx->stream));
+  return B200_OK;
+}
+// fused leaf cliques: CSR of their factors as (group, index), graph order; the BAL point table
+static int setup_leaf_tables(b200_problem* p, ProblemPlan& P) {
+  if (!p->n_fused) return B200_OK;
+  const Symbolic& S = p->sym;
+  const std::vector<int>& fused_list = P.fused_list;
+  std::vector<int> lpos(S.ncliques, -1), fptr(p->n_fused + 1, 0);
+  for (int i = 0; i < p->n_fused; i++) lpos[fused_list[i]] = i;
+  for (int64_t pos = 0; pos < p->nfactors; pos++) if (lpos[S.fac_clique[pos]] >= 0) fptr[lpos[S.fac_clique[pos]] + 1]++;
+  for (int i = 0; i < p->n_fused; i++) fptr[i + 1] += fptr[i];
+  std::vector<int2> ffac(fptr[p->n_fused]);
+  std::vector<int> cur(fptr.begin(), fptr.end() - 1);
+  for (int64_t gi = 0; gi < P.ngroups; gi++)
+    for (int64_t li = 0; li < p->groups[gi].count; li++) {
+      const int64_t pos = p->groups[gi].pos[p->groups[gi].local_index[li]];
+      if (lpos[S.fac_clique[pos]] >= 0) ffac[cur[lpos[S.fac_clique[pos]]]++] = make_int2((int)gi, (int)li);
+    }
+  // keep graph order inside each clique (groups may interleave in the graph; a clique whose factors come from one group
+  // already has it)
+  parallel_chunks(p->n_fused, [&](int64_t i0, int64_t i1, int) {
+    auto gpos = [&](const int2& a) { return p->groups[a.x].pos[p->groups[a.x].local_index[a.y]]; };
+    for (int64_t i = i0; i < i1; i++) {
+      bool ordered = true;
+      for (int q = fptr[i] + 1; q < fptr[i + 1] && ordered; q++) ordered = gpos(ffac[q - 1]) < gpos(ffac[q]);
+      if (!ordered)
+        std::sort(ffac.begin() + fptr[i], ffac.begin() + fptr[i + 1], [&](const int2& a, const int2& b) { return gpos(a) < gpos(b); });
+    }
+  });
+  B200_CUDA(upload(p->d_fused_list, fused_list, p->ctx->stream));
+  B200_CUDA(upload(p->d_fused_run_ptr, P.run_ptr, p->ctx->stream));
+  B200_CUDA(upload(p->d_fused_fac_ptr, fptr, p->ctx->stream));
+  B200_CUDA(upload(p->d_fused_fac, ffac, p->ctx->stream));
+  // BAL point leaves: one flat record per (point position, factor slot 0..7) = (factor index in its group, group << 8 | camera
+  // slot) and the offset of the point's conditional, so that the leaf kernels reach their operands through ONE level of index
+  // loads (list -> fac_ptr -> fac -> scat was a chain of three dependent loads in front of every batch of points)
+  if (p->leaf_pos_end[2] > p->leaf_pos_begin[1] || p->leaf_pos_end[1] > p->leaf_pos_begin[1]) {
+    std::vector<int2> tab((size_t)p->n_fused * kPtMaxObs, make_int2(-1, 0));
+    std::vector<int64_t> poff((size_t)p->n_fused, 0);
     parallel_chunks(p->n_fused, [&](int64_t i0, int64_t i1, int) {
-      auto gpos = [&](const int2& a) { return p->groups[a.x].pos[p->groups[a.x].local_index[a.y]]; };
       for (int64_t i = i0; i < i1; i++) {
-        bool ordered = true;
-        for (int q = fptr[i] + 1; q < fptr[i + 1] && ordered; q++) ordered = gpos(ffac[q - 1]) < gpos(ffac[q]);
-        if (!ordered)
-          std::sort(ffac.begin() + fptr[i], ffac.begin() + fptr[i + 1], [&](const int2& a, const int2& b) { return gpos(a) < gpos(b); });
+        const int c = fused_list[i], kd = P.leaf_kind[c];
+        poff[i] = p->h_off[c];
+        if (kd == 0) continue;
+        const int dc = kd == 1 ? 6 : 9;
+        for (int q = fptr[i]; q < fptr[i + 1]; q++) {
+          const int2 gf = ffac[q];
+          tab[(size_t)i * kPtMaxObs + (q - fptr[i])] = make_int2(gf.y, (gf.x << 8) | ((P.hscat[gf.x][gf.y].y - 3) / dc));
+        }
       }
     });
-    UP(upload(&p->d_fused_list, fused_list, st));
-    UP(upload(&p->d_fused_run_ptr, run_ptr, st));
-    UP(upload(&p->d_fused_fac_ptr, fptr, st));
-    UP(upload(&p->d_fused_fac, ffac, st));
-    // BAL point leaves: one flat record per (point position, factor slot 0..7) = (factor index in its group, group << 8 | camera
-    // slot) and the offset of the point's conditional, so that the leaf kernels reach their operands through ONE level of index
-    // loads (list -> fac_ptr -> fac -> scat was a chain of three dependent loads in front of every batch of points)
-    if (p->leaf_pos_end[2] > p->leaf_pos_begin[1] || p->leaf_pos_end[1] > p->leaf_pos_begin[1]) {
-      std::vector<int2> tab((size_t)p->n_fused * kPtMaxObs, make_int2(-1, 0));
-      std::vector<int64_t> poff((size_t)p->n_fused, 0);
-      parallel_chunks(p->n_fused, [&](int64_t i0, int64_t i1, int) {
-        for (int64_t i = i0; i < i1; i++) {
-          const int c = fused_list[i], kd = leaf_kind[c];
-          poff[i] = p->h_off[c];
-          if (kd == 0) continue;
-          const int dc = kd == 1 ? 6 : 9;
-          for (int q = fptr[i]; q < fptr[i + 1]; q++) {
-            const int2 gf = ffac[q];
-            tab[(size_t)i * kPtMaxObs + (q - fptr[i])] = make_int2(gf.y, (gf.x << 8) | ((hscat[gf.x][gf.y].y - 3) / dc));
-          }
-        }
-      });
-      UP(upload(&p->d_pt_tab, tab, st));
-      UP(upload(&p->d_pt_off, poff, st));
-    }
+    B200_CUDA(upload(p->d_pt_tab, tab, p->ctx->stream));
+    B200_CUDA(upload(p->d_pt_off, poff, p->ctx->stream));
   }
-  lap("leaf factor lists + point table");
-  // ---- level plans: small (one warp per clique) / tile dataflow ----
-  // phase 0: the subtrees this rank owns, leaves to subtree roots; phase 1: the replicated top.
-  // p->levels = [phase-0 levels ..., phase-1 levels ...]; elimination walks it forwards (with the
-  // all-reduce of the top fronts between the phases), back-substitution walks it backwards.
-  std::vector<int> small, bsmall, blarge, bpoint;
+  return B200_OK;
+}
+// Tile grid of a dataflow front: K pivot column blocks of kDfB columns, NB column blocks in all.
+static void df_shape(const Symbolic& S, int c, int& K, int& NB) {
+  const int f = S.nf[c], nn = f + S.ns[c] + 1;
+  K = (f + kDfB - 1) / kDfB; NB = K + (nn - f + kDfB - 1) / kDfB;
+}
+// The number of pivot steps tile (front, column block, row tile) has to see before it is done.
+static int df_need(const Symbolic& S, const int4& t) {
+  int K, NB; df_shape(S, t.x, K, NB);
+  return std::min(K, std::min(std::min(kDfTR * t.z + kDfTR - 1, t.y), NB - 1) + 1);
+}
+// Every wait of front_df_kernel on the tiles T of one launch points to a smaller ticket of that launch (or to an earlier launch).
+static bool df_order_is_safe(const Symbolic& S, const std::vector<int4>& T) {
+  std::vector<int64_t> first(S.ncliques, -1), last(S.ncliques, -1), base(S.ncliques, -1);   // per front: smallest / largest ticket; offset into tk
+  int64_t ntk = 0;
+  for (size_t i = 0; i < T.size(); i++) {
+    const int c = T[i].x;
+    if (base[c] < 0) { int K, NB; df_shape(S, c, K, NB); base[c] = ntk; ntk += (int64_t)NB * ((NB + kDfTR - 1) / kDfTR); first[c] = (int64_t)i; }
+    last[c] = (int64_t)i;
+  }
+  std::vector<int> tk((size_t)ntk, -1);             // ticket of tile (c, j, r)
+  auto slot = [&](int c, int j, int r) { int K, NB; df_shape(S, c, K, NB); return base[c] + (int64_t)j * ((NB + kDfTR - 1) / kDfTR) + r; };
+  for (size_t i = 0; i < T.size(); i++) tk[slot(T[i].x, T[i].y, T[i].z)] = (int)i;
+  for (size_t i = 0; i < T.size(); i++) {
+    const int c = T[i].x, j = T[i].y, r = T[i].z;
+    int K, NB; df_shape(S, c, K, NB);
+    const int last_rb = std::min(std::min(kDfTR * r + kDfTR - 1, j), NB - 1);
+    auto before = [&](int jj, int rr) { const int d = tk[slot(c, jj, rr)]; return (jj == j && rr == r) || (d >= 0 && d < (int)i); };
+    for (int k = 0; k < std::min(K, last_rb + 1); k++) {
+      const int rk = k / kDfTR;
+      if (k <= j && !before(k, rk)) return false;                      // R_kk from the diagonal tile of column k
+      if (rk < r && !before(j, rk)) return false;                      // column piece (k, j)
+      for (int ib = std::max(kDfTR * r, k + 1); ib <= last_rb; ib++)
+        if (ib != j && !before(ib, rk)) return false;                  // row piece (k, ib)
+    }
+    const int par = S.parent[c];
+    if (par >= 0 && first[par] >= 0 && first[par] < last[c]) return false;   // a parent's tiles wait for every tile of its children
+  }
+  return true;
+}
+// What the level planner hands on to the uploads.
+struct LevelLists {
+  std::vector<int> small, bsmall, blarge, bpoint;      // cliques of d_lvl_small / _bsmall / _blarge / _bpoint
+  std::vector<int4> df_tasks[2];                       // per phase: dataflow tiles (front, column block, row tile), ticket order
+  std::vector<int> df_flag_off, df_expect, df_tiles;   // per clique
+  int64_t df_nflags = 0;
+};
+
+// Level plans: small (one warp per clique) / tile dataflow.  Phase 0: the subtrees this rank owns, leaves to subtree roots;
+// phase 1: the replicated top.  p->levels = [phase-0 levels ..., phase-1 levels ...]; elimination walks it forwards (with the
+// all-reduce of the top fronts between the phases), back-substitution walks it backwards.
+static int plan_levels(b200_problem* p, const ProblemPlan& P, LevelLists& L) {
+  const Symbolic& S = p->sym;
   p->levels.resize(2 * S.nlevels);
   p->n_sub_levels = (int)S.nlevels;
   p->max_small_n = 1;
   // tile dataflow (front_df.cuh): per phase, from the first level that holds a front wider than kSmallMaxN upwards,
   // every non-leaf front is a set of tiles of ONE launch; the levels below it (small fronts only) keep elim_small_kernel
   int df_first[2] = {INT_MAX, INT_MAX};
-  std::vector<int4> df_tasks[2];
-  std::vector<int> df_flag_off(S.ncliques, 0), df_expect(S.ncliques, 0), df_tiles(S.ncliques, 0);
-  int64_t df_nflags = 0;
+  L.df_flag_off.assign(S.ncliques, 0); L.df_expect.assign(S.ncliques, 0); L.df_tiles.assign(S.ncliques, 0);
   auto in_phase = [&](int phase, int c) {
-    return phase == 0 ? (!is_top[c] && clique_owner[c] == rank) : (is_top[c] != 0 && (!p->top_staged || top_owner[c] == rank));
+    return phase == 0 ? (!P.is_top[c] && P.clique_owner[c] == p->ctx->rank) : (P.is_top[c] != 0 && (!p->top_staged || P.top_owner[c] == p->ctx->rank));
   };
   for (int phase = 0; phase < 2; phase++)
     for (int64_t c = 0; c < S.ncliques; c++)
-      if (in_phase(phase, (int)c) && !fused[c] && S.nf[c] + S.ns[c] + 1 > kSmallMaxN) df_first[phase] = std::min(df_first[phase], S.level[c]);
+      if (in_phase(phase, (int)c) && !P.fused[c] && S.nf[c] + S.ns[c] + 1 > kSmallMaxN) df_first[phase] = std::min(df_first[phase], S.level[c]);
   if (p->top_staged) df_first[1] = 0;     // every top front goes through its stage's reduce + dataflow launch
   for (int phase = 0; phase < 2; phase++)
   for (int64_t l = 0; l < S.nlevels; l++) {
-    LevelPlan& L = p->levels[phase * S.nlevels + l];
-    L = LevelPlan();
-    L.small_begin = (int)small.size();
-    L.bsmall_begin = (int)bsmall.size();
-    L.blarge_begin = (int)blarge.size();
+    LevelPlan& lv = p->levels[phase * S.nlevels + l];
+    lv = LevelPlan();
+    lv.small_begin = (int)L.small.size();
+    lv.bsmall_begin = (int)L.bsmall.size();
+    lv.blarge_begin = (int)L.blarge.size();
     std::vector<int> pts[2];
-    const size_t stage_task_begin = df_tasks[1].size();
-    const size_t level_task_begin = df_tasks[phase].size();
+    const size_t stage_task_begin = L.df_tasks[1].size();
+    const size_t level_task_begin = L.df_tasks[phase].size();
     for (int64_t q = S.lvl_ptr[l]; q < S.lvl_ptr[l + 1]; q++) {
       const int c = S.lvl_cliques[q];
       const int nn = S.nf[c] + S.ns[c] + 1;
       if (!in_phase(phase, c)) continue;
-      if (fused[c]) {
+      if (P.fused[c]) {
         // eliminated by the leaf kernels; back-substituted 8 lanes per point / one warp per clique
-        if (leaf_kind[c] > 0 && !getenv("B200_NO_POINT_BACKSUB")) pts[leaf_kind[c] - 1].push_back(c);
-        else bsmall.push_back(c);
+        if (P.leaf_kind[c] > 0 && !getenv("B200_NO_POINT_BACKSUB")) pts[P.leaf_kind[c] - 1].push_back(c);
+        else L.bsmall.push_back(c);
       } else if (nn <= kSmallMaxN && l < df_first[phase]) {
-        small.push_back(c);
-        bsmall.push_back(c);
+        L.small.push_back(c);
+        L.bsmall.push_back(c);
         p->max_small_n = std::max(p->max_small_n, nn);
       } else {
-        if (l < df_first[phase]) FAIL(B200_INVALID_ARGUMENT, "level plan: a front wider than kSmallMaxN below the first dataflow level (internal)");
+        if (l < df_first[phase]) { set_error("level plan: a front wider than kSmallMaxN below the first dataflow level (internal)"); return B200_INVALID_ARGUMENT; }
         // tiles (column block j, row tile r) of the upper trapezoid, ticket order: column-major (dependencies point backwards)
-        const int K = (S.nf[c] + kDfB - 1) / kDfB, NB = K + (nn - S.nf[c] + kDfB - 1) / kDfB;
+        int K, NB; df_shape(S, c, K, NB);
         if (p->df_level[phase] < 0) p->df_level[phase] = (int)(phase * S.nlevels + l);
-        df_flag_off[c] = (int)df_nflags;
-        df_nflags += (int64_t)K * NB;
+        L.df_flag_off[c] = (int)L.df_nflags;
+        L.df_nflags += (int64_t)K * NB;
         for (int j = 0; j < NB; j++)
-          for (int r = 0; kDfTR * r <= j; r++) { df_tasks[phase].push_back(make_int4(c, j, r, 0)); df_tiles[c]++; }
-        if (S.parent[c] >= 0) df_expect[S.parent[c]] += df_tiles[c];
-        if (nn <= kSmallMaxN) { bsmall.push_back(c); continue; }
+          for (int r = 0; kDfTR * r <= j; r++) { L.df_tasks[phase].push_back(make_int4(c, j, r, 0)); L.df_tiles[c]++; }
+        if (S.parent[c] >= 0) L.df_expect[S.parent[c]] += L.df_tiles[c];
+        if (nn <= kSmallMaxN) { L.bsmall.push_back(c); continue; }
         // back-substitution cares about the pivots only: thin fronts (<= 8 pivots: one pass of the one-warp kernel
         // over the separator) skip the multi-CTA flag machinery (faster on the BAL trees, about even on sphere2500)
-        if (S.nf[c] <= 8 && !getenv("B200_NO_THIN_BACKSUB")) bsmall.push_back(c);
-        else { blarge.push_back(c); L.blarge_max_nf = std::max(L.blarge_max_nf, S.nf[c]); }
+        if (S.nf[c] <= 8 && !getenv("B200_NO_THIN_BACKSUB")) L.bsmall.push_back(c);
+        else { L.blarge.push_back(c); lv.blarge_max_nf = std::max(lv.blarge_max_nf, S.nf[c]); }
       }
     }
-    L.blarge_count = (int)blarge.size() - L.blarge_begin;
+    lv.blarge_count = (int)L.blarge.size() - lv.blarge_begin;
     for (int kd = 0; kd < 2; kd++) {
-      L.bpoint_begin[kd] = (int)bpoint.size();
-      L.bpoint_count[kd] = (int)pts[kd].size();
-      bpoint.insert(bpoint.end(), pts[kd].begin(), pts[kd].end());
+      lv.bpoint_begin[kd] = (int)L.bpoint.size();
+      lv.bpoint_count[kd] = (int)pts[kd].size();
+      L.bpoint.insert(L.bpoint.end(), pts[kd].begin(), pts[kd].end());
     }
-    L.small_count = (int)small.size() - L.small_begin;
-    L.bsmall_count = (int)bsmall.size() - L.bsmall_begin;
+    lv.small_count = (int)L.small.size() - lv.small_begin;
+    lv.bsmall_count = (int)L.bsmall.size() - lv.bsmall_begin;
     // ticket order inside a level: by column block first, across ALL the level's fronts (then front, row tile).  A tile of column
     // j has nothing to wait for once pivot step j is over, so the resident CTAs (2-3 per SM) are the columns next to every front's
     // pivot — the tiles with work — instead of all the columns of the first few fronts parked on their dependencies while the other
@@ -1507,13 +1525,8 @@ static int create_problem(b200_ctx* ctx, const b200_problem_desc* d, const b200_
       // started late it finds its pieces ready and runs straight through.  A producer never
       // needs more steps than its consumers (smaller-or-equal row tile and column), so the order stays dependency-safe.
       const bool by_need = getenv("B200_DF_NO_NEED_ORDER") == nullptr;
-      auto need = [&](const int4& t) {
-        const int f = S.nf[t.x], nn = f + S.ns[t.x] + 1;
-        const int K = (f + kDfB - 1) / kDfB, NB = K + (nn - f + kDfB - 1) / kDfB;
-        return std::min(K, std::min(std::min(kDfTR * t.z + kDfTR - 1, t.y), NB - 1) + 1);
-      };
-      std::sort(df_tasks[phase].begin() + (int64_t)level_task_begin, df_tasks[phase].end(), [&](const int4& a, const int4& b) {
-        if (by_need) { const int na = need(a), nb = need(b); if (na != nb) return na < nb; }
+      std::sort(L.df_tasks[phase].begin() + (int64_t)level_task_begin, L.df_tasks[phase].end(), [&](const int4& a, const int4& b) {
+        if (by_need) { const int na = df_need(S, a), nb = df_need(S, b); if (na != nb) return na < nb; }
         return a.y != b.y ? a.y < b.y : (a.x != b.x ? a.x < b.x : a.z < b.z); });
     }
     if (phase == 1 && p->top_staged) {
@@ -1522,187 +1535,178 @@ static int create_problem(b200_ctx* ctx, const b200_problem_desc* d, const b200_
       const int64_t x0 = p->topx_doubles;
       for (int64_t q = S.lvl_ptr[l]; q < S.lvl_ptr[l + 1]; q++) {
         const int c = S.lvl_cliques[q];
-        if (!is_top[c]) continue;
+        if (!P.is_top[c]) continue;
         const int64_t nn = S.nf[c] + S.ns[c] + 1;
-        p->ts_fronts.push_back({p->h_off[c], nn * nn, top_owner[c], c});
+        p->ts_fronts.push_back({p->h_off[c], nn * nn, P.top_owner[c], c});
         p->topx_doubles += S.nf[c];
       }
       if ((int)p->ts_fronts.size() > f0) {
         p->ts_level.push_back((int)(S.nlevels + l));
         p->ts_begin.push_back(f0);
         p->ts_task_begin.push_back((int)stage_task_begin);
-        p->ts_task_count.push_back((int)(df_tasks[1].size() - stage_task_begin));
+        p->ts_task_count.push_back((int)(L.df_tasks[1].size() - stage_task_begin));
         p->ts_x_begin.push_back((int)x0);
         p->ts_x_count.push_back((int)(p->topx_doubles - x0));
       }
     }
   }
   p->ts_begin.push_back((int)p->ts_fronts.size());
-  {
-    // Ticket order across levels (B200_DF_ORDER=1, the default; 0 = level by level): by the ESTIMATED time a tile can finish, in pivot
-    // steps — its front's start (= the latest finish of a child front) + the pivot steps it has to see; trailing-column tiles
-    // optionally B200_DF_LAG steps later (they then find their pieces ready instead of idling on a slot).  A front whose
-    // children are done early no longer waits for the tickets of the rest of its level.  Dependency-safe: a producer's key
-    // is never larger than its consumer's (same front: fewer steps, pivot columns before trailing ones; children: finish
-    // <= the parent's start), ties broken as before — and df_order_is_safe() below checks the result, whatever the order.
-    const int df_order = getenv("B200_DF_ORDER") ? atoi(getenv("B200_DF_ORDER")) : 1;
-    const int df_lag = getenv("B200_DF_LAG") ? std::max(0, atoi(getenv("B200_DF_LAG"))) : 2;
-    auto shape = [&](int c, int& K, int& NB) {
-      const int f = S.nf[c], nn = f + S.ns[c] + 1;
-      K = (f + kDfB - 1) / kDfB; NB = K + (nn - f + kDfB - 1) / kDfB;
-    };
-    auto need_of = [&](const int4& t) {
-      int K, NB; shape(t.x, K, NB);
-      return std::min(K, std::min(std::min(kDfTR * t.z + kDfTR - 1, t.y), NB - 1) + 1);
-    };
-    if (df_order >= 1) {
-      std::vector<int64_t> est(S.ncliques, 0);
-      for (int64_t c = 0; c < S.ncliques; c++) {      // children have smaller ids than parents
-        if (!df_tiles[c] || S.parent[c] < 0) continue;
-        int K, NB; shape((int)c, K, NB);
-        est[S.parent[c]] = std::max(est[S.parent[c]], est[c] + K + 1 + df_lag);
-      }
-      for (int phase = 0; phase < 2; phase++) {
-        if (phase == 1 && p->top_staged) continue;     // the staged top is launched level by level
-        auto key = [&](const int4& t) { int K, NB; shape(t.x, K, NB); return est[t.x] + need_of(t) + (t.y >= K ? df_lag : 0); };
-        std::sort(df_tasks[phase].begin(), df_tasks[phase].end(), [&](const int4& a, const int4& b) {
-          const int64_t ka = key(a), kb = key(b);
-          if (ka != kb) return ka < kb;
-          const int na = need_of(a), nb = need_of(b);
-          if (na != nb) return na < nb;
-          return a.y != b.y ? a.y < b.y : (a.x != b.x ? a.x < b.x : a.z < b.z); });
-      }
-    }
-    // every wait of front_df_kernel must point to a smaller ticket of the same launch (or to an earlier launch)
-    for (int phase = 0; phase < 2; phase++) {
-      const std::vector<int4>& T = df_tasks[phase];
-      std::vector<int64_t> first(S.ncliques, -1), base(S.ncliques, -1);   // per front: smallest ticket; offset into tk
-      std::vector<int64_t> last(S.ncliques, -1);
-      int64_t ntk = 0;
-      for (size_t i = 0; i < T.size(); i++) {
-        const int c = T[i].x;
-        if (base[c] < 0) { int K, NB; shape(c, K, NB); base[c] = ntk; ntk += (int64_t)NB * ((NB + kDfTR - 1) / kDfTR); first[c] = (int64_t)i; }
-        last[c] = (int64_t)i;
-      }
-      std::vector<int> tk((size_t)ntk, -1);             // ticket of tile (c, j, r)
-      auto slot = [&](int c, int j, int r) { int K, NB; shape(c, K, NB); return base[c] + (int64_t)j * ((NB + kDfTR - 1) / kDfTR) + r; };
-      for (size_t i = 0; i < T.size(); i++) tk[slot(T[i].x, T[i].y, T[i].z)] = (int)i;
-      bool safe = true;
-      for (size_t i = 0; i < T.size() && safe; i++) {
-        const int c = T[i].x, j = T[i].y, r = T[i].z;
-        int K, NB; shape(c, K, NB);
-        const int last_rb = std::min(std::min(kDfTR * r + kDfTR - 1, j), NB - 1);
-        for (int k = 0; k < std::min(K, last_rb + 1) && safe; k++) {
-          const int rk = k / kDfTR;
-          auto before = [&](int jj, int rr) { const int d = tk[slot(c, jj, rr)]; return (jj == j && rr == r) || (d >= 0 && d < (int)i); };
-          if (k <= j && !before(k, rk)) safe = false;                      // R_kk from the diagonal tile of column k
-          if (rk < r && !before(j, rk)) safe = false;                      // column piece (k, j)
-          for (int ib = std::max(kDfTR * r, k + 1); ib <= last_rb && safe; ib++)
-            if (ib != j && !before(ib, rk)) safe = false;                  // row piece (k, ib)
-        }
-        const int par = S.parent[c];
-        if (par >= 0 && first[par] >= 0 && first[par] < last[c]) safe = false;   // a parent's tiles wait for every tile of its children
-      }
-      if (!safe) FAIL(B200_INVALID_ARGUMENT, "front dataflow: ticket order is not dependency-safe (internal)");
-    }
+  return B200_OK;
+}
+// Ticket order across levels (B200_DF_ORDER=1, the default; 0 = level by level): by the ESTIMATED time a tile can finish, in pivot
+// steps — its front's start (= the latest finish of a child front) + the pivot steps it has to see; trailing-column tiles
+// optionally B200_DF_LAG steps later (they then find their pieces ready instead of idling on a slot).  A front whose
+// children are done early no longer waits for the tickets of the rest of its level.  Dependency-safe: a producer's key
+// is never larger than its consumer's (same front: fewer steps, pivot columns before trailing ones; children: finish
+// <= the parent's start), ties broken as before — and df_order_is_safe() checks the result, whatever the order.
+static void order_tickets(const b200_problem* p, LevelLists& L) {
+  const Symbolic& S = p->sym;
+  const int df_order = getenv("B200_DF_ORDER") ? atoi(getenv("B200_DF_ORDER")) : 1;
+  const int df_lag = getenv("B200_DF_LAG") ? std::max(0, atoi(getenv("B200_DF_LAG"))) : 2;
+  if (df_order < 1) return;
+  std::vector<int64_t> est(S.ncliques, 0);
+  for (int64_t c = 0; c < S.ncliques; c++) {      // children have smaller ids than parents
+    if (!L.df_tiles[c] || S.parent[c] < 0) continue;
+    int K, NB; df_shape(S, (int)c, K, NB);
+    est[S.parent[c]] = std::max(est[S.parent[c]], est[c] + K + 1 + df_lag);
   }
+  for (int phase = 0; phase < 2; phase++) {
+    if (phase == 1 && p->top_staged) continue;     // the staged top is launched level by level
+    auto key = [&](const int4& t) { int K, NB; df_shape(S, t.x, K, NB); return est[t.x] + df_need(S, t) + (t.y >= K ? df_lag : 0); };
+    std::sort(L.df_tasks[phase].begin(), L.df_tasks[phase].end(), [&](const int4& a, const int4& b) {
+      const int64_t ka = key(a), kb = key(b);
+      if (ka != kb) return ka < kb;
+      const int na = df_need(S, a), nb = df_need(S, b);
+      if (na != nb) return na < nb;
+      return a.y != b.y ? a.y < b.y : (a.x != b.x ? a.x < b.x : a.z < b.z); });
+  }
+}
+static int setup_levels(b200_problem* p, ProblemPlan& P) {
+  const Symbolic& S = p->sym;
+  LevelLists L;
+  if (const int rc = plan_levels(p, P, L)) return rc;
+  order_tickets(p, L);
+  for (int phase = 0; phase < 2; phase++)
+    if (!df_order_is_safe(S, L.df_tasks[phase])) { set_error("front dataflow: ticket order is not dependency-safe (internal)"); return B200_INVALID_ARGUMENT; }
   if (p->top_staged && !p->ts_fronts.empty()) {
     std::vector<int> tc, tx, to;
     int64_t x = 0;
-    for (auto& tf : p->ts_fronts) { tc.push_back(tf.clique); tx.push_back((int)x); to.push_back(tf.owner == rank ? 1 : 0); x += S.nf[tf.clique]; }
-    UP(upload(&p->d_ts_cliques, tc, st));
-    UP(upload(&p->d_ts_xoff, tx, st));
-    UP(upload(&p->d_ts_owned, to, st));
-    B200_CUDA(cudaMalloc((void**)&p->d_topx, (size_t)std::max<int64_t>(1, p->topx_doubles) * sizeof(double)));
+    for (auto& tf : p->ts_fronts) { tc.push_back(tf.clique); tx.push_back((int)x); to.push_back(tf.owner == p->ctx->rank ? 1 : 0); x += S.nf[tf.clique]; }
+    B200_CUDA(upload(p->d_ts_cliques, tc, p->ctx->stream));
+    B200_CUDA(upload(p->d_ts_xoff, tx, p->ctx->stream));
+    B200_CUDA(upload(p->d_ts_owned, to, p->ctx->stream));
+    B200_CUDA(p->d_topx.alloc(p->topx_doubles));
   }
-  if (df_nflags + S.ncliques + 4 * (S.nlevels + 2) > (int64_t)INT_MAX) FAIL(B200_INVALID_ARGUMENT, "front dataflow: flag table exceeds 2^31 entries");
+  if (L.df_nflags + S.ncliques + 4 * (S.nlevels + 2) > (int64_t)INT_MAX) { set_error("front dataflow: flag table exceeds 2^31 entries"); return B200_INVALID_ARGUMENT; }
   for (int phase = 0; phase < 2; phase++) {
-    p->df_ntasks[phase] = (int)df_tasks[phase].size();
-    if (p->df_ntasks[phase]) UP(upload(&p->d_df_tasks[phase], df_tasks[phase], st));
+    p->df_ntasks[phase] = (int)L.df_tasks[phase].size();
+    if (p->df_ntasks[phase]) B200_CUDA(upload(p->d_df_tasks[phase], L.df_tasks[phase], p->ctx->stream));
   }
   // backsub_large_kernel solves with the diagonal-block inverses W that front_df_kernel leaves behind
-  for (int c : blarge)
-    if (!df_tiles[c]) FAIL(B200_INVALID_ARGUMENT, "level plan: a multi-CTA back-substitution front without diagonal-block inverses (internal)");
+  for (int c : L.blarge)
+    if (!L.df_tiles[c]) { set_error("level plan: a multi-CTA back-substitution front without diagonal-block inverses (internal)"); return B200_INVALID_ARGUMENT; }
   if (p->df_ntasks[0] + p->df_ntasks[1]) {
     std::vector<int64_t> woff(S.ncliques, -1);
     int64_t wtot = 0;
     for (int64_t c = 0; c < S.ncliques; c++)
-      if (df_tiles[c]) { woff[c] = wtot; wtot += (int64_t)((S.nf[c] + kDfB - 1) / kDfB) * kDfB * kDfB; }
-    UP(upload(&p->d_winv_off, woff, st));
-    B200_CUDA(cudaMalloc((void**)&p->d_winv, (size_t)std::max<int64_t>(1, wtot) * sizeof(double)));
-    UP(upload(&p->d_df_flag_off, df_flag_off, st));
-    UP(upload(&p->d_df_expect, df_expect, st));
+      if (L.df_tiles[c]) { woff[c] = wtot; wtot += (int64_t)((S.nf[c] + kDfB - 1) / kDfB) * kDfB * kDfB; }
+    B200_CUDA(upload(p->d_winv_off, woff, p->ctx->stream));
+    B200_CUDA(p->d_winv.alloc(wtot));
+    B200_CUDA(upload(p->d_df_flag_off, L.df_flag_off, p->ctx->stream));
+    B200_CUDA(upload(p->d_df_expect, L.df_expect, p->ctx->stream));
     p->df_ctrl_ints = 2 * (2 + (int)S.nlevels);     // (ticket, abort) per launch: the two phases + one per stage of the top
-    p->df_sync_ints = p->df_ctrl_ints + S.ncliques + df_nflags;
+    p->df_sync_ints = p->df_ctrl_ints + S.ncliques + L.df_nflags;
     // latency variant (2 CTAs per SM, 252 registers) unless the tree has more tiles than that keeps busy
-    p->df_minb = (p->df_ntasks[0] + p->df_ntasks[1] > 6 * ctx->sm_count) ? 3 : 2;
+    p->df_minb = (p->df_ntasks[0] + p->df_ntasks[1] > 6 * p->ctx->sm_count) ? 3 : 2;
     if (const char* e = getenv("B200_DF_MINB")) p->df_minb = atoi(e) == 3 ? 3 : 2;
-    B200_CUDA(cudaMalloc((void**)&p->d_df_sync, (size_t)p->df_sync_ints * sizeof(int)));
-#ifndef B200_EMULATE
-    B200_CUDA(cudaFuncSetAttribute(front_df_kernel<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, kDfSmemBytes));
-    B200_CUDA(cudaFuncSetAttribute(front_df_kernel<3>, cudaFuncAttributeMaxDynamicSharedMemorySize, kDfSmemBytes));
-#endif
+    B200_CUDA(p->d_df_sync.alloc(p->df_sync_ints));
     if (getenv("B200_DF_TRACE") && p->df_ntasks[0]) {
-      B200_CUDA(cudaMalloc((void**)&p->d_df_trace, (size_t)p->df_ntasks[0] * 32 * 8));
-      B200_CUDA(cudaMemsetAsync(p->d_df_trace, 0, (size_t)p->df_ntasks[0] * 32 * 8, st));
+      B200_CUDA(p->d_df_trace.alloc((size_t)p->df_ntasks[0] * 32));
+      B200_CUDA(cudaMemsetAsync(p->d_df_trace, 0, (size_t)p->df_ntasks[0] * 32 * 8, p->ctx->stream));
     }
   }
-  UP(upload(&p->d_lvl_small, small, st));
-  UP(upload(&p->d_lvl_bsmall, bsmall, st));
-  UP(upload(&p->d_lvl_blarge, blarge, st));
-  UP(upload(&p->d_lvl_bpoint, bpoint, st));
-  {
-    std::vector<int> fbase(blarge.size() + 1, 0);
-    for (size_t i = 0; i < blarge.size(); i++) fbase[i + 1] = fbase[i] + (S.nf[blarge[i]] + kBsRows - 1) / kBsRows;
-    UP(upload(&p->d_bs_flag_base, fbase, st));
-    p->n_bs_flags = fbase.back();
-    B200_CUDA(cudaMalloc((void**)&p->d_bs_flags, (size_t)std::max(1, fbase.back()) * sizeof(int)));
-    B200_CUDA(cudaMemsetAsync(p->d_bs_flags, 0, (size_t)std::max(1, fbase.back()) * sizeof(int), st));
-  }
-  lap("level plans + dataflow tickets");
-  // ---- values views (sharded problems move only what a rank needs / owns between host and device) ----
-  if (d) {
-    std::vector<char> need(n, ctx->world == 1), own(n, ctx->world == 1);
-    if (ctx->world > 1) {
-      for (int64_t c = 0; c < S.ncliques; c++) {
-        const bool mine = is_top[c] ? true : clique_owner[c] == rank;
-        if (!mine) continue;
-        for (int64_t q = S.front_ptr[c]; q < S.front_ptr[c + 1]; q++) {
-          need[S.front_vars[q]] = 1;
-          if (!is_top[c] || rank == 0) own[S.front_vars[q]] = 1;     // the top's variables are reported by rank 0
-        }
+  B200_CUDA(upload(p->d_lvl_small, L.small, p->ctx->stream));
+  B200_CUDA(upload(p->d_lvl_bsmall, L.bsmall, p->ctx->stream));
+  B200_CUDA(upload(p->d_lvl_blarge, L.blarge, p->ctx->stream));
+  B200_CUDA(upload(p->d_lvl_bpoint, L.bpoint, p->ctx->stream));
+  std::vector<int> fbase(L.blarge.size() + 1, 0);
+  for (size_t i = 0; i < L.blarge.size(); i++) fbase[i + 1] = fbase[i] + (S.nf[L.blarge[i]] + kBsRows - 1) / kBsRows;
+  B200_CUDA(upload(p->d_bs_flag_base, fbase, p->ctx->stream));
+  p->n_bs_flags = fbase.back();
+  B200_CUDA(p->d_bs_flags.alloc(fbase.back()));
+  B200_CUDA(cudaMemsetAsync(p->d_bs_flags, 0, (size_t)std::max(1, fbase.back()) * sizeof(int), p->ctx->stream));
+  return B200_OK;
+}
+// values views (sharded problems move only what a rank needs / owns between host and device)
+static int setup_values_views(b200_problem* p, ProblemPlan& P) {
+  if (!P.d) return B200_OK;
+  const Symbolic& S = p->sym;
+  const int64_t n = p->nvars;
+  const int world = p->ctx->world;
+  std::vector<char> need(n, world == 1), own(n, world == 1);
+  if (world > 1) {
+    for (int64_t c = 0; c < S.ncliques; c++) {
+      if (!P.is_top[c] && P.clique_owner[c] != p->ctx->rank) continue;
+      for (int64_t q = S.front_ptr[c]; q < S.front_ptr[c + 1]; q++) {
+        need[S.front_vars[q]] = 1;
+        if (!P.is_top[c] || p->ctx->rank == 0) own[S.front_vars[q]] = 1;     // the top's variables are reported by rank 0
       }
-      for (int64_t gi = 0; gi < ngroups; gi++)
-        for (auto& k : hkeys[gi]) { need[k.x] = 1; if (k.y >= 0) need[k.y] = 1; }
     }
-    for (int w = 0; w < 2; w++) {
-      const std::vector<char>& m = w == 0 ? need : own;
-      std::vector<int> idx;
-      for (int64_t v = 0; v < n; v++)
-        if (m[v]) { p->view_vars[w].push_back(v); for (int k = val_off[v]; k < val_off[v + 1]; k++) idx.push_back(k); }
-      p->view_doubles[w] = (int64_t)idx.size();
-      UP(upload(&p->d_view_idx[w], idx, st));
-    }
-    B200_CUDA(cudaMalloc((void**)&p->d_view_buf, (size_t)std::max<int64_t>(1, std::max(p->view_doubles[0], p->view_doubles[1])) * sizeof(double)));
+    for (int64_t gi = 0; gi < P.ngroups; gi++)
+      for (auto& k : P.hkeys[gi]) { need[k.x] = 1; if (k.y >= 0) need[k.y] = 1; }
   }
-  // ---- arena + scratch ----
-  B200_CUDA(cudaMalloc((void**)&p->d_arena, std::max<int64_t>(1, p->arena_doubles) * sizeof(double)));
-  p->partial_cap = 2 * ctx->sm_count * 8;
-  B200_CUDA(cudaMalloc((void**)&p->d_partials, (size_t)p->partial_cap * sizeof(double)));
-  B200_CUDA(cudaMalloc((void**)&p->d_counters, 4 * sizeof(unsigned)));
-  B200_CUDA(cudaMemsetAsync(p->d_counters, 0, 4 * sizeof(unsigned), st));
-  B200_CUDA(cudaMalloc((void**)&p->d_scalars, sizeof(Scalars)));
-  B200_CUDA(cudaMemsetAsync(p->d_scalars, 0, sizeof(Scalars), st));
-  B200_CUDA(cudaMallocHost((void**)&p->h_scalars, sizeof(Scalars)));
-  B200_CUDA(cudaMalloc((void**)&p->d_lambda, sizeof(double)));
-  B200_CUDA(cudaMemsetAsync(p->d_lambda, 0, sizeof(double), st));
-  B200_CUDA(cudaMallocHost((void**)&p->h_lambda, sizeof(double)));
-  B200_CUDA(cudaMallocHost((void**)&p->h_pinned, std::max<int64_t>(81, std::max(p->nval, p->ndelta)) * sizeof(double)));   // >= 9 x 9: one marginal covariance
-  B200_CUDA(cudaStreamSynchronize(st));
-#undef FAIL
-#undef UP
+  for (int w = 0; w < 2; w++) {
+    const std::vector<char>& m = w == 0 ? need : own;
+    std::vector<int> idx;
+    for (int64_t v = 0; v < n; v++)
+      if (m[v]) { p->view_vars[w].push_back(v); for (int k = P.pk.val_off[v]; k < P.pk.val_off[v + 1]; k++) idx.push_back(k); }
+    p->view_doubles[w] = (int64_t)idx.size();
+    B200_CUDA(upload(p->d_view_idx[w], idx, p->ctx->stream));
+  }
+  B200_CUDA(p->d_view_buf.alloc(std::max(p->view_doubles[0], p->view_doubles[1])));
+  return B200_OK;
+}
+static int setup_scratch(b200_problem* p, ProblemPlan& P) {
+  B200_CUDA(p->d_arena.alloc(p->arena_doubles));
+  p->partial_cap = 2 * p->ctx->sm_count * 8;
+  B200_CUDA(p->d_partials.alloc(p->partial_cap));
+  B200_CUDA(p->d_counters.alloc(4));
+  B200_CUDA(cudaMemsetAsync(p->d_counters, 0, 4 * sizeof(unsigned), p->ctx->stream));
+  B200_CUDA(p->d_scalars.alloc(1));
+  B200_CUDA(cudaMemsetAsync(p->d_scalars, 0, sizeof(Scalars), p->ctx->stream));
+  B200_CUDA(p->h_scalars.alloc(1));
+  B200_CUDA(p->d_lambda.alloc(1));
+  B200_CUDA(cudaMemsetAsync(p->d_lambda, 0, sizeof(double), p->ctx->stream));
+  B200_CUDA(p->h_lambda.alloc(1));
+  B200_CUDA(p->h_pinned.alloc(std::max<int64_t>(81, std::max(p->nval, p->ndelta))));   // >= 9 x 9: one marginal covariance
+  return B200_OK;
+}
+// Problem creation, shared by the two descriptions: `d` (nonlinear graph + Values, b200_problem_create) or
+// `ld` (JacobianFactors, b200_linear_create); exactly one of them is non-null.
+static int create_problem(b200_ctx* ctx, const b200_problem_desc* d, const b200_linear_desc* ld, b200_problem** out) {
+  if (!ctx || (!d && !ld) || !out) { set_error("null argument"); return B200_INVALID_ARGUMENT; }
+  B200_CUDA(cudaSetDevice(ctx->device));
+  std::unique_ptr<b200_problem, int (*)(b200_problem*)> p(new b200_problem(), b200_problem_destroy);   // freed on every early return
+  p->ctx = ctx; p->linear = ld != nullptr;
+  ProblemPlan P{d, ld};
+  // B200_SETUP_TIMING=1: where the one-time setup goes (host wall clock per named stage, stderr)
+  static const struct { int (*run)(b200_problem*, ProblemPlan&); const char* name; } stages[] = {
+      {setup_symbolic, "validate + symbolic phase"}, {setup_values, "values + variable tables"}, {setup_leaf_runs, "shard plan + leaf runs"},
+      {setup_offsets, "front offsets"}, {setup_linear_groups, nullptr}, {setup_typed_groups, "factor tables"}, {setup_tree_tables, "tree tables"},
+      {setup_leaf_tables, "leaf factor lists + point table"}, {setup_levels, "level plans + dataflow tickets"},
+      {setup_values_views, nullptr}, {setup_scratch, nullptr}};
+  const bool setup_timing = getenv("B200_SETUP_TIMING") != nullptr;
+  auto t_prev = std::chrono::steady_clock::now();
+  for (const auto& s : stages) {
+    if (const int rc = s.run(p.get(), P)) return rc;
+    if (!setup_timing || !s.name) continue;
+    const auto now = std::chrono::steady_clock::now();
+    fprintf(stderr, "[b200 setup] %-28s %8.1f ms\n", s.name, std::chrono::duration<double, std::milli>(now - t_prev).count());
+    t_prev = now;
+  }
+  B200_CUDA(cudaStreamSynchronize(ctx->stream));
   p->linearized = p->linear;   // a linear problem IS its linearization
-  *out = p;
+  *out = p.release();
   return B200_OK;
 }
 
@@ -1724,22 +1728,14 @@ static int upload_jacobian_group(b200_problem* p, b200_problem::Group& g, const 
       sigmas = own_sig.data();
     }
   }
-  double *d_stage = nullptr, *d_sig = nullptr;
-  B200_CUDA(cudaMalloc((void**)&d_stage, nel * sizeof(double)));
-  cudaError_t ce = cudaMemcpyAsync(d_stage, Ab, nel * sizeof(double), cudaMemcpyHostToDevice, st);
-  if (ce == cudaSuccess && sigmas) {
-    ce = cudaMalloc((void**)&d_sig, (size_t)g.count * g.d * sizeof(double));
-    if (ce == cudaSuccess) ce = cudaMemcpyAsync(d_sig, sigmas, (size_t)g.count * g.d * sizeof(double), cudaMemcpyHostToDevice, st);
-  }
-  if (ce == cudaSuccess) {
-    const int nb = (int)std::min<int64_t>(((int64_t)nel + 255) / 256, (int64_t)p->ctx->sm_count * 16);
-    launch_plain(jacobian_load_kernel, dim3(nb), dim3(256), 0, st, (const double*)d_stage, (const double*)d_sig, g.d, g.ncols, (int)g.count, g.d_J);
-    p->ctx->launches++;
-    ce = cudaGetLastError();
-  }
-  if (ce == cudaSuccess) ce = cudaStreamSynchronize(st);   // the caller's buffers and the staging copies die with this call
-  cudaFree(d_stage); cudaFree(d_sig);
-  if (ce != cudaSuccess) { set_error(std::string("upload_jacobian_group: ") + cudaGetErrorString(ce)); return B200_CUDA_ERROR; }
+  DevPtr<double> d_stage, d_sig;
+  B200_CUDA(upload(d_stage, Ab, nel, st));
+  if (sigmas) B200_CUDA(upload(d_sig, sigmas, (size_t)g.count * g.d, st));
+  const int nb = (int)std::min<int64_t>(((int64_t)nel + 255) / 256, (int64_t)p->ctx->sm_count * 16);
+  launch_plain(jacobian_load_kernel, dim3(nb), dim3(256), 0, st, (const double*)d_stage, (const double*)d_sig, g.d, g.ncols, (int)g.count, g.d_J);
+  p->ctx->launches++;
+  B200_CUDA(cudaGetLastError());
+  B200_CUDA(cudaStreamSynchronize(st));   // the caller's buffers and the staging copies die with this call
   return B200_OK;
 }
 
@@ -1815,15 +1811,12 @@ int b200_set_group_noise(b200_problem* p, int64_t group, int32_t noise_kind, int
   } else {
     h.assign(noise, noise + payload);
   }
-  double* fresh = nullptr;
-  int rc = upload(&fresh, h, p->ctx->stream);
-  if (rc) return rc;
+  DevPtr<double> fresh;
+  B200_CUDA(upload(fresh, h, p->ctx->stream));
   B200_CUDA(cudaStreamSynchronize(p->ctx->stream));   // h goes out of scope
-  cudaFree(g.d_noise);
-  g.d_noise = fresh;
+  g.d_noise = std::move(fresh);
   g.noise_kind = noise_kind; g.per_factor = noise_per_factor ? 1 : 0; g.noise_size = payload;
-  for (int i = 0; i < 2; i++)   // the captured LM try has the group views baked in
-    if (p->try_graph[i]) { cudaGraphExecDestroy(p->try_graph[i]); p->try_graph[i] = nullptr; }
+  drop_try_graphs(p);
   p->linearized = p->solved = p->factored = p->marg_ready = false;
   return B200_OK;
 }
@@ -1872,7 +1865,7 @@ int b200_get_values_all(b200_problem* p, double* v) {
   if (p->ctx->world <= 1) return b200_get_values(p, v);
   B200_CUDA(cudaSetDevice(p->ctx->device));
   cudaStream_t st = p->ctx->stream;
-  if (!p->d_gather_buf) B200_CUDA(cudaMalloc((void**)&p->d_gather_buf, (size_t)std::max<int64_t>(1, p->nval) * sizeof(double)));
+  if (!p->d_gather_buf) B200_CUDA(p->d_gather_buf.alloc(p->nval));
   B200_CUDA(cudaMemsetAsync(p->d_gather_buf, 0, (size_t)p->nval * sizeof(double), st));
   const int64_t nd = p->view_doubles[1];
   launch_plain(values_view_kernel, dim3((unsigned)((nd + 255) / 256)), dim3(256), 0, st, p->d_values, p->d_gather_buf, (const int*)p->d_view_idx[1], nd, 2);
@@ -1951,13 +1944,12 @@ int b200_set_jacobian_precision(b200_problem* p, int fp32) {
   if (want == p->jac_f32) return B200_OK;
   B200_CUDA(cudaSetDevice(p->ctx->device));
   B200_CUDA(cudaStreamSynchronize(p->ctx->stream));
-  for (auto& g : p->groups) {   // re-allocate at the new element size (the old contents are a stale linearization anyway)
-    cudaFree(g.d_J);
-    g.d_J = nullptr;
-    B200_CUDA(cudaMalloc((void**)&g.d_J, std::max<size_t>(1, (size_t)g.count * g.d * g.ncols) * (want ? sizeof(float) : sizeof(double))));
-  }
-  for (int i = 0; i < 2; i++)   // the captured LM try has the buffers and kernel instantiations baked in
-    if (p->try_graph[i]) { cudaGraphExecDestroy(p->try_graph[i]); p->try_graph[i] = nullptr; }
+  // re-allocate at the new element size (the old contents are a stale linearization anyway); on failure nothing changes
+  std::vector<DevPtr<double>> fresh(p->groups.size());
+  for (size_t i = 0; i < fresh.size(); i++)
+    B200_CUDA(fresh[i].alloc((size_t)p->groups[i].count * p->groups[i].d * p->groups[i].ncols, want ? sizeof(float) : sizeof(double)));
+  for (size_t i = 0; i < fresh.size(); i++) p->groups[i].d_J = std::move(fresh[i]);
+  drop_try_graphs(p);
   p->jac_f32 = want;
   p->linearized = p->solved = p->factored = p->marg_ready = false;
   return B200_OK;
@@ -1976,8 +1968,7 @@ int b200_set_tuning(b200_problem* p, const char* key, int64_t value) {
   else { set_error("b200_set_tuning: unknown key " + k); return B200_INVALID_ARGUMENT; }
   B200_CUDA(cudaSetDevice(p->ctx->device));
   B200_CUDA(cudaStreamSynchronize(p->ctx->stream));
-  for (int i = 0; i < 2; i++)   // the captured LM try has the kernel instantiations baked in
-    if (p->try_graph[i]) { cudaGraphExecDestroy(p->try_graph[i]); p->try_graph[i] = nullptr; }
+  drop_try_graphs(p);
   return B200_OK;
 }
 
@@ -1999,7 +1990,7 @@ int b200_gradient_at_zero(b200_problem* p, double* out) {
   if (!p->linearized) { set_error("b200_gradient_at_zero before b200_linearize"); return B200_INVALID_ARGUMENT; }
   B200_CUDA(cudaSetDevice(p->ctx->device));
   cudaStream_t st = p->ctx->stream;
-  if (!p->d_grad) B200_CUDA(cudaMalloc((void**)&p->d_grad, (size_t)std::max<int64_t>(1, p->ndelta) * sizeof(double)));
+  if (!p->d_grad) B200_CUDA(p->d_grad.alloc(p->ndelta));
   double* grad = p->d_grad;
   B200_CUDA(cudaMemsetAsync(grad, 0, (size_t)p->ndelta * sizeof(double), st));
   for (auto& g : p->groups) {
@@ -2031,7 +2022,7 @@ int b200_linear_graph_error(b200_problem* p, const double* x, double* err) {
   if (!p->linearized) { set_error("b200_linear_graph_error before b200_linearize"); return B200_INVALID_ARGUMENT; }
   B200_CUDA(cudaSetDevice(p->ctx->device));
   cudaStream_t st = p->ctx->stream;
-  if (!p->d_grad) B200_CUDA(cudaMalloc((void**)&p->d_grad, (size_t)std::max<int64_t>(1, p->ndelta) * sizeof(double)));
+  if (!p->d_grad) B200_CUDA(p->d_grad.alloc(p->ndelta));
   memcpy(p->h_pinned, x, (size_t)p->ndelta * sizeof(double));
   B200_CUDA(cudaMemcpyAsync(p->d_grad, p->h_pinned, (size_t)p->ndelta * sizeof(double), cudaMemcpyHostToDevice, st));
   int rc = enqueue_linerr_of(p, p->d_grad, 1.0, &p->d_scalars->graph_err);
@@ -2107,7 +2098,7 @@ int b200_accept_step(b200_problem* p) {
 int b200_save_values(b200_problem* p) {
   if (p->linear) { set_error("this call needs Values: not available on a linear problem (b200_linear_create)"); return B200_INVALID_ARGUMENT; }
   B200_CUDA(cudaSetDevice(p->ctx->device));
-  if (!p->d_saved_values) B200_CUDA(cudaMalloc((void**)&p->d_saved_values, std::max<int64_t>(1, p->nval) * sizeof(double)));
+  if (!p->d_saved_values) B200_CUDA(p->d_saved_values.alloc(p->nval));
   B200_CUDA(cudaMemcpyAsync(p->d_saved_values, p->d_values, (size_t)p->nval * sizeof(double), cudaMemcpyDeviceToDevice, p->ctx->stream));
   return B200_OK;
 }
@@ -2138,8 +2129,8 @@ int b200_profile_enable(b200_problem* p, int on) {
 int b200_measure_fp64_peak(b200_ctx* ctx, double* dmma_tflops, double* dfma_tflops) {
   if (!ctx || !dmma_tflops || !dfma_tflops) { set_error("null argument"); return B200_INVALID_ARGUMENT; }
   B200_CUDA(cudaSetDevice(ctx->device));
-  double* sink = nullptr;
-  B200_CUDA(cudaMalloc((void**)&sink, sizeof(double)));
+  DevPtr<double> sink;
+  B200_CUDA(sink.alloc(1));
   cudaEvent_t e0, e1;
   cudaEventCreate(&e0); cudaEventCreate(&e1);
   const int iters = 4096, blocks = ctx->sm_count * 8;
@@ -2159,7 +2150,6 @@ int b200_measure_fp64_peak(b200_ctx* ctx, double* dmma_tflops, double* dfma_tflo
       ctx->launches++;
     }
   cudaEventDestroy(e0); cudaEventDestroy(e1);
-  cudaFree(sink);
   if (getenv("B200_PEAK_VERBOSE"))
     fprintf(stderr, "[b200 fp64 peak] m16n8k16 %.1f, m8n8k4 %.1f, FMA %.1f TFLOP/s\n", best[2], best[1], best[0]);
   *dmma_tflops = std::max(best[1], best[2]); *dfma_tflops = best[0];
@@ -2517,11 +2507,9 @@ int b200_marginal_covariance(b200_problem* p, int64_t var, double* out) {
   }
   const int d = (int)(S.var_dof[var + 1] - S.var_dof[var]);
   if (d > 9) { set_error("b200_marginal_covariance: variable dimension > 9 (use b200_joint_marginal_covariance)"); return B200_INVALID_ARGUMENT; }
-  if (!p->d_marg_work) {
-    B200_CUDA(cudaMalloc((void**)&p->d_marg_work, (size_t)9 * std::max<int64_t>(1, p->ndelta) * sizeof(double)));
-    B200_CUDA(cudaMalloc((void**)&p->d_marg_path, (size_t)std::max<int64_t>(1, S.ncliques) * sizeof(int)));
-    B200_CUDA(cudaMalloc((void**)&p->d_marg_out, 81 * sizeof(double)));
-  }
+  if (!p->d_marg_work) B200_CUDA(p->d_marg_work.alloc((size_t)9 * std::max<int64_t>(1, p->ndelta)));
+  if (!p->d_marg_path) B200_CUDA(p->d_marg_path.alloc(S.ncliques));
+  if (!p->d_marg_out) B200_CUDA(p->d_marg_out.alloc(81));
   B200_CUDA(cudaMemcpyAsync(p->d_marg_path, path.data(), path.size() * sizeof(int), cudaMemcpyHostToDevice, st));
   B200_CUDA(cudaStreamSynchronize(st));   // `path` is pageable and dies with this call
   launch_plain(marginal_path_kernel, dim3(d), dim3(256), 0, st, tview(p), (const int*)p->d_marg_path, (int)path.size(), (int)S.var_dof[var], d,
@@ -2561,51 +2549,41 @@ int b200_joint_marginal_covariance(b200_problem* p, const int64_t* vars, int64_t
   std::vector<int> path;
   for (int c = 0; c < (int)S.ncliques; c++)
     if (on[c]) path.push_back(c);   // ascending clique id = elimination order
-  double *d_work = nullptr, *d_out = nullptr;
-  int *d_path = nullptr, *d_dofs = nullptr;
-  B200_CUDA(cudaMalloc((void**)&d_work, (size_t)D * std::max<int64_t>(1, p->ndelta) * sizeof(double)));
-  B200_CUDA(cudaMalloc((void**)&d_out, (size_t)D * D * sizeof(double)));
-  B200_CUDA(cudaMalloc((void**)&d_path, path.size() * sizeof(int)));
-  B200_CUDA(cudaMalloc((void**)&d_dofs, (size_t)D * sizeof(int)));
-  B200_CUDA(cudaMemcpyAsync(d_path, path.data(), path.size() * sizeof(int), cudaMemcpyHostToDevice, st));
-  B200_CUDA(cudaMemcpyAsync(d_dofs, dofs.data(), (size_t)D * sizeof(int), cudaMemcpyHostToDevice, st));
+  DevPtr<double> d_work, d_out;
+  DevPtr<int> d_path, d_dofs;
+  B200_CUDA(d_work.alloc((size_t)D * std::max<int64_t>(1, p->ndelta)));
+  B200_CUDA(d_out.alloc((size_t)D * D));
+  B200_CUDA(upload(d_path, path, st));
+  B200_CUDA(upload(d_dofs, dofs, st));
   B200_CUDA(cudaStreamSynchronize(st));
   launch_plain(marginal_joint_kernel, dim3(D), dim3(256), 0, st, tview(p), (const int*)d_path, (int)path.size(), (const int*)d_dofs, D, d_work,
                p->ndelta, d_out);
   ctx->launches++;
-  cudaError_t ce = cudaGetLastError();
-  if (ce == cudaSuccess) ce = cudaMemcpyAsync(out, d_out, (size_t)D * D * sizeof(double), cudaMemcpyDeviceToHost, st);
-  if (ce == cudaSuccess) ce = cudaStreamSynchronize(st);
-  cudaFree(d_work); cudaFree(d_out); cudaFree(d_path); cudaFree(d_dofs);
-  if (ce != cudaSuccess) { set_error(std::string("b200_joint_marginal_covariance: ") + cudaGetErrorString(ce)); return B200_CUDA_ERROR; }
+  B200_CUDA(cudaGetLastError());
+  B200_CUDA(cudaMemcpyAsync(out, d_out, (size_t)D * D * sizeof(double), cudaMemcpyDeviceToHost, st));
+  B200_CUDA(cudaStreamSynchronize(st));
   return B200_OK;
 }
 
 // ---- Dogleg ------------------------------------------------------------------------------
-int b200_dl_destroy(b200_dl* dl);
 int b200_dl_create(b200_problem* p, double delta_initial, b200_dl** out) {
   // the sharded solve leaves each rank with its own slice of delta; Dogleg's global dot products
   // over dx_u / dx_n are not wired for that layout
   if (p->ctx->world > 1) { set_error("Dogleg is single-GPU: create the problem on a context without a communicator"); return B200_INVALID_ARGUMENT; }
   if (p->linear) { set_error("this call needs Values: not available on a linear problem (b200_linear_create)"); return B200_INVALID_ARGUMENT; }
   B200_CUDA(cudaSetDevice(p->ctx->device));
-  b200_dl* dl = new b200_dl;
+  std::unique_ptr<b200_dl> dl(new b200_dl);
   dl->prob = p;
   dl->delta = delta_initial;
   dl->iterations = 0;
-  B200_CUDA(cudaMalloc((void**)&dl->d_grad, (size_t)std::max<int64_t>(1, p->ndelta) * sizeof(double)));
-  B200_CUDA(cudaMalloc((void**)&dl->d_dxn, (size_t)std::max<int64_t>(1, p->ndelta) * sizeof(double)));
-  int rc = b200_error(p, &dl->error);
-  if (rc) { b200_dl_destroy(dl); return rc; }
-  *out = dl;
+  B200_CUDA(dl->d_grad.alloc(p->ndelta));
+  B200_CUDA(dl->d_dxn.alloc(p->ndelta));
+  const int rc = b200_error(p, &dl->error);
+  if (rc) return rc;
+  *out = dl.release();
   return B200_OK;
 }
-int b200_dl_destroy(b200_dl* dl) {
-  if (!dl) return B200_OK;
-  cudaFree(dl->d_grad); cudaFree(dl->d_dxn);
-  delete dl;
-  return B200_OK;
-}
+int b200_dl_destroy(b200_dl* dl) { delete dl; return B200_OK; }
 int b200_dl_get_state(const b200_dl* dl, double* error, double* delta, int32_t* iterations) {
   if (error) *error = dl->error;
   if (delta) *delta = dl->delta;

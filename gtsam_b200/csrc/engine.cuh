@@ -2,6 +2,7 @@
 #pragma once
 #include <cuda_runtime.h>
 
+#include <algorithm>
 #include <cstdint>
 #include <string>
 #include <vector>
@@ -22,6 +23,30 @@ void set_error(const std::string& s);
       return B200_CUDA_ERROR;                                                             \
     }                                                                                     \
   } while (0)
+
+// Sole, move-only owner of one device allocation (Host = true: page-locked host memory), freed when the owner is destroyed,
+// reassigned or reallocated.  Converts to the raw pointer, so kernel arguments and pointer arithmetic take it as they are.
+template <class T, bool Host = false>
+class DevPtr {
+  T* p_ = nullptr;
+ public:
+  DevPtr() = default;
+  DevPtr(DevPtr&& o) noexcept : p_(o.p_) { o.p_ = nullptr; }
+  DevPtr& operator=(DevPtr&& o) noexcept { T* q = o.p_; o.p_ = nullptr; reset(); p_ = q; return *this; }
+  ~DevPtr() { reset(); }
+  // max(n, 1) elements of `elem` bytes (FP32 Jacobian storage keeps floats in a DevPtr<double>)
+  cudaError_t alloc(size_t n, size_t elem = sizeof(T)) {
+    reset();
+    void* q = nullptr;
+    const cudaError_t e = Host ? cudaMallocHost(&q, std::max<size_t>(n, 1) * elem) : cudaMalloc(&q, std::max<size_t>(n, 1) * elem);
+    if (e == cudaSuccess) p_ = (T*)q;
+    return e;
+  }
+  void reset() { if (p_) Host ? cudaFreeHost(p_) : cudaFree(p_); p_ = nullptr; }
+  T* get() const { return p_; }
+  operator T*() const { return p_; }
+  T* operator->() const { return p_; }
+};
 
 // Device-side view of one factor group (passed to kernels by value).
 struct GroupView {
@@ -90,6 +115,7 @@ struct LevelPlan {
 }  // namespace b200
 
 namespace b200 { struct ncclUniqueIdBlob { char internal[128]; }; }
+using b200::DevPtr;
 
 struct b200_ctx {
   int rank = 0, world = 1;   // one process per GPU; world > 1 after b200_ctx_comm_init
@@ -114,54 +140,50 @@ struct b200_problem {
     double robust_param = 0;
     int64_t count;
     std::vector<int64_t> pos;          // graph position of every factor of the caller's group
-    int2* d_keys = nullptr;
-    double* d_meas = nullptr;
-    double* d_noise = nullptr;
-    int* d_cal = nullptr;
-    double* d_body = nullptr;
-    double* d_J = nullptr;
-    int4* d_scat = nullptr;
+    DevPtr<int2> d_keys;
+    DevPtr<double> d_meas, d_noise, d_body, d_J;
+    DevPtr<int> d_cal;
+    DevPtr<int4> d_scat;
     int col0[B200_JACOBIAN_MAX_ARITY + 2] = {0};   // JacobianFactor groups: first column of every block
-    int *d_jkeys = nullptr, *d_jslots = nullptr, *d_jclique = nullptr;   // JacobianFactor groups (see JacobianView)
+    DevPtr<int> d_jkeys, d_jslots, d_jclique;   // JacobianFactor groups (see JacobianView)
     int64_t n_nonleaf = 0;   // factors NOT owned by a fused leaf clique
     std::vector<int64_t> local_index;  // index in the caller's group of every factor kept on this rank
     int64_t full_count = 0;            // linear groups: the caller's factor count (count = this rank's share)
   };
   std::vector<Group> groups;
   // device state
-  double *d_values = nullptr, *d_new_values = nullptr, *d_delta = nullptr, *d_hdiag = nullptr;
-  double* d_grad = nullptr;          // b200_gradient_at_zero (allocated on first use)
-  int *d_val_off = nullptr, *d_var_type = nullptr, *d_var_dof = nullptr;
-  double* d_cal = nullptr;
-  double* d_arena = nullptr;
-  int64_t* d_off = nullptr;
-  int *d_nf = nullptr, *d_ns = nullptr, *d_parent = nullptr, *d_ld = nullptr;
+  DevPtr<double> d_values, d_new_values, d_delta, d_hdiag;
+  DevPtr<double> d_grad;             // b200_gradient_at_zero (allocated on first use)
+  DevPtr<int> d_val_off, d_var_type, d_var_dof;
+  DevPtr<double> d_cal, d_arena;
+  DevPtr<int64_t> d_off;
+  DevPtr<int> d_nf, d_ns, d_parent, d_ld;
   std::vector<int64_t> h_off;       // final arena offsets (fused leaves store f x n only)
   std::vector<int> h_ld;
   // fused leaf path
-  int n_fused = 0, n_runs = 0, leaf_lb_cap = 1, leaf_acc_cap = 0;
+  int n_fused = 0, n_runs = 0, leaf_lb_cap = 1;
   int leaf_run_begin[3] = {0, 0, 0}, leaf_run_end[3] = {0, 0, 0};  // run ranges: generic / point DC=6 / point DC=9
   int schur_pb = 4;                                                 // points per staged batch of leaf_point_schur_kernel
   bool schur_mma = true;                                            // BAL point leaves: factor + per-run Schur complement on the FP64 tensor path in one kernel (leaf_point_fused_mma_kernel)
   int lin_variant = 0;                                              // linearize_kernel variant of the projection groups (b200_set_tuning)
   int leaf_max_w[3] = {1, 1, 1};                                    // widest separator + 1 per kind
   int leaf_pos_begin[3] = {0, 0, 0}, leaf_pos_end[3] = {0, 0, 0};  // the same ranges as positions in d_fused_list
-  int *d_fused_list = nullptr, *d_fused_fac_ptr = nullptr, *d_fused_run_ptr = nullptr;
-  int2* d_fused_fac = nullptr;
-  int2* d_pt_tab = nullptr;         // BAL point leaves: per (list position, factor slot) (factor index, group << 8 | camera slot); -1: no factor
-  int64_t* d_pt_off = nullptr;      // ... and the arena offset of the point's conditional
+  DevPtr<int> d_fused_list, d_fused_fac_ptr, d_fused_run_ptr;
+  DevPtr<int2> d_fused_fac;
+  DevPtr<int2> d_pt_tab;            // BAL point leaves: per (list position, factor slot) (factor index, group << 8 | camera slot); -1: no factor
+  DevPtr<int64_t> d_pt_off;         // ... and the arena offset of the point's conditional
   int64_t top_doubles = 0;          // [0, top_doubles) = fronts of the replicated top (all-reduced when sharded)
   int n_sub_levels = 0;             // levels[0..n_sub_levels) = owned subtrees, the rest = the top
   int64_t arena_doubles = 0, zero_doubles = 0;  // [0, zero_doubles) = non-leaf fronts (memset per solve)
-  int64_t *d_ea_ptr = nullptr, *d_didx_ptr = nullptr;
-  int *d_ea_map = nullptr, *d_didx = nullptr;
-  int64_t* d_diag_index = nullptr;  // per delta scalar: arena index of its diagonal entry
-  int *d_lvl_small = nullptr, *d_lvl_bsmall = nullptr, *d_lvl_blarge = nullptr, *d_lvl_bpoint = nullptr;
+  DevPtr<int64_t> d_ea_ptr, d_didx_ptr;
+  DevPtr<int> d_ea_map, d_didx;
+  DevPtr<int64_t> d_diag_index;     // per delta scalar: arena index of its diagonal entry
+  DevPtr<int> d_lvl_small, d_lvl_bsmall, d_lvl_blarge, d_lvl_bpoint;
   std::vector<b200::LevelPlan> levels;
-  int *d_bs_flags = nullptr, *d_bs_flag_base = nullptr;  // publish flags of the multi-CTA back-substitution
+  DevPtr<int> d_bs_flags, d_bs_flag_base;  // publish flags of the multi-CTA back-substitution
   int n_bs_flags = 0;
-  double* d_lambda = nullptr;       // lambda of the current try (device resident)
-  double* h_lambda = nullptr;       // pinned
+  DevPtr<double> d_lambda;          // lambda of the current try (device resident)
+  DevPtr<double, true> h_lambda;   // pinned
   cudaGraphExec_t try_graph[2] = {nullptr, nullptr};  // LM try (solve + retract + error), by diagonal flag
   double graph_min_diag[2] = {0, 0}, graph_max_diag[2] = {0, 0};
   bool hdiag_valid = false;         // d_hdiag holds hessianDiagonal of the current linearization
@@ -169,46 +191,46 @@ struct b200_problem {
   // tile-dataflow elimination of the non-leaf fronts (front_df.cuh): one launch per phase (own subtrees / replicated top)
   int df_level[2] = {-1, -1};       // index in `levels` at which the launch of the phase is issued
   int df_ntasks[2] = {0, 0};
-  int4* d_df_tasks[2] = {nullptr, nullptr};
-  int *d_df_flag_off = nullptr, *d_df_expect = nullptr;
-  int* d_df_sync = nullptr;         // [ctrl of phase 0 (2) | ctrl of phase 1 (2) | done per clique | piece flags]: zeroed per solve
+  DevPtr<int4> d_df_tasks[2];
+  DevPtr<int> d_df_flag_off, d_df_expect;
+  DevPtr<int> d_df_sync;            // [ctrl of phase 0 (2) | ctrl of phase 1 (2) | done per clique | piece flags]: zeroed per solve
   int64_t df_sync_ints = 0;
   int df_ctrl_ints = 4;
   int df_minb = 3;                  // kernel variant: resident CTAs per SM it is compiled for
-  unsigned long long* d_df_trace = nullptr;   // B200_DF_TRACE: 32 globaltimer stamps per tile of phase 0
+  DevPtr<unsigned long long> d_df_trace;      // B200_DF_TRACE: 32 globaltimer stamps per tile of phase 0
   // sharded solve, distributed top (DESIGN.md 7): every front of the top of the tree has an OWNER rank; per top level
   // ("stage") the ranks' partial fronts are summed onto their owners (ncclReduce, grouped), the owners factor them
   // (front_df_kernel over their tiles of the stage) and extend-add into their copy of the parent; back-substitution
   // walks the stages downwards, the owners' solutions travel in a packed vector (one small all-reduce per stage)
-  double* d_winv = nullptr;         // W = R_kk^-1 of every factored 32 x 32 diagonal block (front_df_kernel), for back-substitution
-  int64_t* d_winv_off = nullptr;    // per clique: offset into d_winv (-1: none)
+  DevPtr<double> d_winv;            // W = R_kk^-1 of every factored 32 x 32 diagonal block (front_df_kernel), for back-substitution
+  DevPtr<int64_t> d_winv_off;       // per clique: offset into d_winv (-1: none)
   // values views of a sharded problem (b200_values_view): [0] what this rank needs as input, [1] what it owns
   std::vector<int64_t> view_vars[2];
   int64_t view_doubles[2] = {0, 0};
-  int* d_view_idx[2] = {nullptr, nullptr};   // per packed double: its index in the full packed Values
-  double* d_view_buf = nullptr;
-  double* d_gather_buf = nullptr;            // b200_get_values_all: full-size buffer the owned views are all-reduced in
+  DevPtr<int> d_view_idx[2];                 // per packed double: its index in the full packed Values
+  DevPtr<double> d_view_buf;
+  DevPtr<double> d_gather_buf;               // b200_get_values_all: full-size buffer the owned views are all-reduced in
   bool defer_scalar_reduce = false; // inside an LM try: the scalar all-reduces are merged into one (enqueue_try)
-  double* d_red = nullptr;
+  DevPtr<double> d_red;
   bool top_staged = false;
   struct TopFront { int64_t off, count; int owner, clique; };
   std::vector<TopFront> ts_fronts;              // all top fronts, grouped by stage
   std::vector<int> ts_level, ts_begin, ts_task_begin, ts_task_count, ts_x_begin, ts_x_count;   // per stage (ts_begin has nstages + 1 entries)
-  int *d_ts_cliques = nullptr, *d_ts_xoff = nullptr, *d_ts_owned = nullptr;
-  double* d_topx = nullptr;
+  DevPtr<int> d_ts_cliques, d_ts_xoff, d_ts_owned;
+  DevPtr<double> d_topx;
   int64_t topx_doubles = 0;
-  double* d_partials = nullptr;     // block partial sums
-  unsigned* d_counters = nullptr;   // tickets of the last-block reductions
+  DevPtr<double> d_partials;        // block partial sums
+  DevPtr<unsigned> d_counters;      // tickets of the last-block reductions
   int partial_cap = 0;
-  b200::Scalars* d_scalars = nullptr;
-  b200::Scalars* h_scalars = nullptr;  // pinned
-  double* h_pinned = nullptr;          // pinned staging for values
+  DevPtr<b200::Scalars> d_scalars;
+  DevPtr<b200::Scalars, true> h_scalars;   // pinned
+  DevPtr<double, true> h_pinned;           // pinned staging for values
   bool linearized = false, solved = false, factored = false;
   bool marg_ready = false;          // the fronts hold the UNDAMPED factor of H at the current values
-  double* d_marg_work = nullptr;    // Marginals: one scratch vector per covariance column
-  int* d_marg_path = nullptr;
-  double* d_marg_out = nullptr;
-  double* d_saved_values = nullptr;
+  DevPtr<double> d_marg_work;       // Marginals: one scratch vector per covariance column
+  DevPtr<int> d_marg_path;
+  DevPtr<double> d_marg_out;
+  DevPtr<double> d_saved_values;
   // phase timers
   bool profile = false;
   std::vector<std::pair<cudaEvent_t, cudaEvent_t>> ev_pool;
@@ -224,8 +246,8 @@ struct b200_dl {
   double delta;        // trust region radius (DoglegState::delta)
   double error;
   int iterations;
-  double* d_grad = nullptr;   // gradientAtZero, then scaled in the blend
-  double* d_dxn = nullptr;    // Newton point
+  DevPtr<double> d_grad;   // gradientAtZero, then scaled in the blend
+  DevPtr<double> d_dxn;    // Newton point
 };
 
 struct b200_lm {

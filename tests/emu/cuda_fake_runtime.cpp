@@ -15,10 +15,22 @@ cudaError_t cudaGetDeviceProperties_v2(cudaDeviceProp* p, int) { memset(p, 0, si
 cudaError_t cudaStreamCreateWithFlags(cudaStream_t* s, unsigned) { *s = (cudaStream_t)0x1; return cudaSuccess; }
 cudaError_t cudaStreamDestroy(cudaStream_t) { return cudaSuccess; }
 cudaError_t cudaStreamSynchronize(cudaStream_t) { return cudaSuccess; }
-cudaError_t cudaMalloc(void** p, size_t n) { *p = calloc(n ? n : 1, 1); return *p ? cudaSuccess : cudaErrorMemoryAllocation; }
-cudaError_t cudaFree(void* p) { free(p); return cudaSuccess; }
+// allocation-failure injection (tests/emu/run_scenarios.py allocfail): the live count of cudaMalloc / cudaMallocHost blocks,
+// and a countdown after which one allocation fails
+static long g_live = 0, g_fail_in = 0;
+long b200_emu_live_allocs(void) { return g_live; }
+void b200_emu_fail_alloc_in(long k) { g_fail_in = k; }   // the k-th next allocation fails (k >= 1); 0: none
+cudaError_t cudaMalloc(void** p, size_t n) {
+  *p = nullptr;
+  if (g_fail_in > 0 && --g_fail_in == 0) return cudaErrorMemoryAllocation;
+  *p = calloc(n ? n : 1, 1);
+  if (!*p) return cudaErrorMemoryAllocation;
+  g_live++;
+  return cudaSuccess;
+}
+cudaError_t cudaFree(void* p) { if (p) g_live--; free(p); return cudaSuccess; }
 cudaError_t cudaMallocHost(void** p, size_t n) { return cudaMalloc(p, n); }
-cudaError_t cudaFreeHost(void* p) { free(p); return cudaSuccess; }
+cudaError_t cudaFreeHost(void* p) { return cudaFree(p); }
 cudaError_t cudaMemcpyAsync(void* d, const void* s, size_t n, cudaMemcpyKind, cudaStream_t) { if (n) memmove(d, s, n); return cudaSuccess; }
 cudaError_t cudaMemcpy(void* d, const void* s, size_t n, cudaMemcpyKind k) { return cudaMemcpyAsync(d, s, n, k, 0); }
 cudaError_t cudaMemsetAsync(void* d, int v, size_t n, cudaStream_t) { if (n) memset(d, v, n); return cudaSuccess; }

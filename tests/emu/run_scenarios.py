@@ -454,7 +454,74 @@ def coverage(_):
             os.environ.pop("B200_DF_ORDER"); os.environ.pop("B200_DF_LAG")
 
 
-SCEN = dict(coverage=coverage, leafshapes=leafshapes, midsize=midsize, edge=edge, bigfront=bigfront, gnc=gnc_scenario, typed=typed, fp32=fp32, linear=linear, marginals=marginals, dogleg=dogleg, gn=gn, mirror=linear_mirror)
+def allocfail(_):
+    """Each allocation a call makes fails in turn (tests/emu/cuda_fake_runtime.cpp): the call returns B200_CUDA_ERROR and
+    leaves as many blocks allocated as there were before it; b200_set_jacobian_precision leaves the problem as it was."""
+    import ctypes as C
+    from gtsam_b200 import datasets
+    L = ctx.L
+    L.b200_emu_live_allocs.restype = C.c_long
+    L.b200_emu_fail_alloc_in.argtypes = [C.c_long]
+
+    def each_failure(what, call, after=None):
+        k = 0
+        while True:
+            k += 1
+            live = L.b200_emu_live_allocs()
+            L.b200_emu_fail_alloc_in(k)
+            rc = call()
+            L.b200_emu_fail_alloc_in(0)
+            if rc == P.OK:
+                break
+            assert rc == P.CUDA_ERROR, (what, k, rc)
+            assert L.b200_emu_live_allocs() == live, (what, "allocation %d failed" % k, L.b200_emu_live_allocs() - live, "blocks leaked")
+            if after:
+                after()
+        assert k > 1, (what, "no allocation")
+
+    def create(what, fn, desc):
+        def call():
+            h = C.c_void_p()
+            live = L.b200_emu_live_allocs()
+            rc = fn(ctx.h, C.byref(desc), C.byref(h))
+            if rc == P.OK:
+                L.b200_problem_destroy(h)
+                assert L.b200_emu_live_allocs() == live, (what, "b200_problem_destroy")
+            return rc
+        each_failure(what, call)
+
+    for name, prob in (("bal_small_metis", util.load_case("bal_small_metis")), ("bigfront", datasets.make("sphere_tiny", layers=10, per_ring=16))):
+        desc, keep = prob.c_desc()
+        create(name, L.b200_problem_create, desc)
+    lp = util.load_linear_case("lin_random_nary")
+    desc, keep = lp.c_desc()
+    create("lin_random_nary", L.b200_linear_create, desc)
+    prob = util.load_case("bal_tiny_s2")
+    dev = capi.DeviceProblem(ctx, prob)
+
+    def dl_create():
+        h = C.c_void_p()
+        rc = L.b200_dl_create(dev.h, 1.0, C.byref(h))
+        if rc == P.OK:
+            L.b200_dl_destroy(h)
+        return rc
+    each_failure("b200_dl_create", dl_create)
+    vs, cov = np.array([0, 1], dtype=np.int64), np.zeros(128 * 128)
+    joint = lambda: L.b200_joint_marginal_covariance(dev.h, vs.ctypes.data_as(C.POINTER(C.c_int64)), 2, cov.ctypes.data_as(C.POINTER(C.c_double)))  # noqa: E731
+    assert joint() == P.OK     # (the marginals' own buffers, kept by the problem, exist from here on)
+    each_failure("b200_joint_marginal_covariance", joint)
+
+    def unchanged():
+        assert L.b200_get_jacobian_precision(dev.h) == 0
+        dev.restore_values()      # (the dump check accepts a step)
+        util.check_against_dump(dev, prob, util.golden("bal_tiny_s2", "dump1"), 1e-2, 1)
+    dev.save_values()
+    each_failure("b200_set_jacobian_precision", lambda: L.b200_set_jacobian_precision(dev.h, 1), unchanged)
+    assert L.b200_get_jacobian_precision(dev.h) == 1
+    dev.close()
+
+
+SCEN = dict(allocfail=allocfail, coverage=coverage, leafshapes=leafshapes, midsize=midsize, edge=edge, bigfront=bigfront, gnc=gnc_scenario, typed=typed, fp32=fp32, linear=linear, marginals=marginals, dogleg=dogleg, gn=gn, mirror=linear_mirror)
 for arg in sys.argv[2:]:
     kind, case = arg.split(":")
     t = time.time()

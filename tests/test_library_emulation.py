@@ -46,6 +46,8 @@ GROUPS = [
     ["edge:x", "coverage:x", "midsize:cal3_s2", "midsize:bundler", "midsize:bundler@8", "midsize:cal3_s2@8", "midsize:bundler@4", "midsize:cal3_s2@5", "midsize:bundler@3", "bigfront:x"],
     # the BAL point leaves at mixed separator widths and run lengths (tests/test_point_leaf_shapes.py)
     ["leafshapes:cal3_s2", "leafshapes:bundler"],
+    # every allocation of problem creation, Dogleg, joint marginals and the Jacobian storage switch failing in turn: nothing leaks
+    ["allocfail:x"],
     # the GaussianFactorGraph level, Dogleg, Gauss-Newton
     ["linear:" + c for c in ("lin_pose2_toy", "lin_pose2_synth", "lin_random_nary", "lin_mixed_hessian", "lin_arity8", "lin_sphere_tiny",
                              "lin_bal_tiny", "lin_singular", "lin_family_sfm2", "lin_family_smart", "lin_family_expr")] +
