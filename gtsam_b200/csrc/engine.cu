@@ -289,9 +289,10 @@ static int enqueue_solve(b200_problem* p, bool damped, int diagonal, double min_
       const int mmax = std::max(1, (maxw - 1) / dc), sa = (dc < 8 ? 8 : 16) * kSmPA + kSmPadA;
       const size_t jb = p->jac_f32 ? sizeof(float) : sizeof(double);
       // leaf_point_fused_mma_kernel's layout: per warp [R S' d']^T, then per warp [A_c b]^T (two buffers) and A_p (two
-      // buffers); the four warps' Schur sums (8 nt8)^2 reuse it at the end
+      // buffers); the four warps' partial sums (8x8 tiles of -S'^T S' and of every camera's [A_c b]^T [A_c b]) reuse it at the end
+      const int ct = dc < 8 ? 1 : 2;
       const size_t sm = std::max((size_t)4 * (3 + 8 * nt8) * kSmKS * sizeof(double) + (size_t)4 * (2 * mmax * sa + 2 * 6 * 32) * jb,
-                                 (size_t)64 * nt8 * nt8 * sizeof(double));
+                                 (size_t)4 * 64 * (nt8 * (nt8 + 1) / 2 + mmax * ct * (ct + 1) / 2) * sizeof(double));
       bool done = false;
 #define B200_LAUNCH_FUSED(DC_, T_)                                                                                                    \
       if (!done && dc == DC_ && nt8 <= T_) {                                                                                          \
@@ -1156,16 +1157,50 @@ static int setup_leaf_runs(b200_problem* p, ProblemPlan& P) {
     return s != 0 ? s < 0 : a < b;
   });
   const int nfl = (int)fused_list.size();
-  // long enough to amortise the per-run extend-add, short enough for >= 8 CTAs per SM
-  int run_max_pt = getenv("B200_NO_LEAF_RUNS") ? 1 : std::max(1, std::min(64, nfl / (ctx->sm_count * 8)));
-  if (getenv("B200_LEAF_RUN_MAX")) run_max_pt = std::max(1, atoi(getenv("B200_LEAF_RUN_MAX")));
+  // shared memory per warp of the generic leaf kernel: the widest [F S d] block
+  for (int c : fused_list) {
+    if (kind[c] == 0) p->leaf_lb_cap = std::max(p->leaf_lb_cap, S.nf[c] * (S.nf[c] + S.ns[c] + 1));
+    p->leaf_max_w[kind[c]] = std::max(p->leaf_max_w[kind[c]], S.ns[c] + 1);
+  }
+  // Leaf runs.  A camera set (the BAL points of one kind with one run signature) is cut into runs as long as the kind still
+  // fills kLeafRunWaves waves of the CTAs its instantiation of leaf_point_fused_mma_kernel keeps resident, but no shorter
+  // than min(64, points / (8 SMs)); the cuts split a set evenly.  A run pays a fixed cost that does not overlap with its
+  // streaming (index loads, the reduction of the four warps' sums, the extend-add), so the longest runs that still fill the
+  // GPU stream fastest (DESIGN.md 5c).  B200_LEAF_RUN_MAX cuts at a fixed length instead (L + L + ... + rest), and
+  // B200_NO_LEAF_RUNS makes every point a run of its own; every other leaf clique is a run of its own.
+  constexpr int kLeafRunWaves = 3;
+  std::vector<int> set_ptr(1, 0);
+  for (int i = 1; i <= nfl; i++)
+    if (i == nfl || kind[fused_list[i - 1]] == 0 || kind[fused_list[i]] != kind[fused_list[i - 1]] || sig_cmp(fused_list[i - 1], fused_list[i]) != 0)
+      set_ptr.push_back(i);
+  const char* run_max_env = getenv("B200_LEAF_RUN_MAX");
+  const bool fixed_runs = run_max_env || getenv("B200_NO_LEAF_RUNS");
+  int run_len[3] = {1, 1, 1};
+  for (int kd = 1; kd <= 2; kd++) {
+    std::vector<int> n;
+    for (size_t q = 0; q + 1 < set_ptr.size(); q++) if (kind[fused_list[set_ptr[q]]] == kd) n.push_back(set_ptr[q + 1] - set_ptr[q]);
+    if (n.empty() || getenv("B200_NO_LEAF_RUNS")) continue;
+    if (run_max_env) { run_len[kd] = std::max(1, atoi(run_max_env)); continue; }
+    const int64_t target = (int64_t)kLeafRunWaves * ctx->sm_count * leaf_point_fused_min_blocks(kd == 1 ? 6 : 9, (p->leaf_max_w[kd] + 7) / 8);
+    auto runs = [&](int len) { int64_t r = 0; for (int x : n) r += (x + len - 1) / len; return r; };
+    int lo = std::max(1, std::min(64, nfl / (ctx->sm_count * 8))), hi = *std::max_element(n.begin(), n.end());
+    while (lo < hi) {            // the longest run length that still gives target runs (the floor when none does)
+      const int mid = lo + (hi - lo + 1) / 2;
+      if (runs(mid) >= target) lo = mid; else hi = mid - 1;
+    }
+    run_len[kd] = lo;
+  }
   std::vector<int>& run_ptr = P.run_ptr;
   run_ptr.push_back(0);
-  for (int i = 1; i <= nfl; i++) {
-    const int kprev = kind[fused_list[i - 1]];
-    const int rmax = kprev == 0 ? 1 : run_max_pt;
-    if (i == nfl || i - run_ptr.back() >= rmax || kind[fused_list[i]] != kprev || sig_cmp(fused_list[i - 1], fused_list[i]) != 0)
-      run_ptr.push_back(i);
+  for (size_t q = 0; q + 1 < set_ptr.size(); q++) {
+    const int i0 = set_ptr[q], n = set_ptr[q + 1] - i0, len = run_len[kind[fused_list[i0]]];
+    if (fixed_runs) {
+      for (int i = i0 + len; i < i0 + n; i += len) run_ptr.push_back(i);
+      run_ptr.push_back(i0 + n);
+    } else {
+      const int k = (n + len - 1) / len;
+      for (int r = 1; r <= k; r++) run_ptr.push_back(i0 + (int)((int64_t)n * r / k));
+    }
   }
   p->n_runs = (int)run_ptr.size() - 1;
   for (int kd = 0, r = 0; kd < 3; kd++) {
@@ -1174,11 +1209,6 @@ static int setup_leaf_runs(b200_problem* p, ProblemPlan& P) {
     p->leaf_run_end[kd] = r;
     p->leaf_pos_begin[kd] = run_ptr[p->leaf_run_begin[kd]];
     p->leaf_pos_end[kd] = run_ptr[r];
-  }
-  // shared memory per warp of the generic leaf kernel: the widest [F S d] block
-  for (int c : fused_list) {
-    if (kind[c] == 0) p->leaf_lb_cap = std::max(p->leaf_lb_cap, S.nf[c] * (S.nf[c] + S.ns[c] + 1));
-    p->leaf_max_w[kind[c]] = std::max(p->leaf_max_w[kind[c]], S.ns[c] + 1);
   }
   p->n_fused = nfl;
   p->schur_pb = (getenv("B200_SCHUR_PB") && atoi(getenv("B200_SCHUR_PB")) == 6) ? 6 : 4;

@@ -1178,9 +1178,11 @@ constexpr int kSmPA = 12;
 constexpr int kSmPadA = 4;               // behind every camera's [A_c b]^T block: the 8 cameras of a factor-phase access hit
                                          // different banks (2 wavefronts per float access instead of 8)
 
-// (min. 3 blocks = 168 registers at 6 dofs and up to 40 columns: at 4 blocks = 128 registers the factorisation spills)
+// CTAs per SM an instantiation is compiled for (min. 3 blocks = 168 registers at 6 dofs and up to 40 columns: at 4 blocks
+// = 128 registers the factorisation spills); the run planner (engine.cu) sizes the runs from it
+constexpr int leaf_point_fused_min_blocks(int dc, int ntt) { return (ntt <= 5 && dc == 6) ? 3 : (ntt <= 7 ? 2 : 1); }
 template <int DC, int NTT, typename JT = double>   // NTT: 8-column strips of the widest separator (+ rhs column) of the kind
-__global__ void __launch_bounds__(128, (NTT <= 5 && DC == 6) ? 3 : (NTT <= 7 ? 2 : 1))
+__global__ void __launch_bounds__(128, leaf_point_fused_min_blocks(DC, NTT))
 leaf_point_fused_mma_kernel(TreeView t, GroupTable gt, const int* __restrict__ list, const int* __restrict__ run_ptr,
                             const double* __restrict__ lambda_ptr, const double* __restrict__ hdiag, double min_diag,
                             double max_diag, Scalars* sc, const int2* __restrict__ pt_tab, const int64_t* __restrict__ pt_off) {
@@ -1202,6 +1204,8 @@ leaf_point_fused_mma_kernel(TreeView t, GroupTable gt, const int* __restrict__ l
   const int s = t.ns[c0], w = s + 1;
   const int m = s / DC;                                       // one factor per separator camera
   const int NT = (w + 7) >> 3, WP = 8 * NT;
+  __shared__ int sMap[8 * NTT];                               // the run's extend-add map (read after the last barrier)
+  if (tid < w) { const int pp = t.parent[c0]; if (pp >= 0) sMap[tid] = t.ea_map[t.ea_ptr[c0] + tid]; }
   const int f_doubles = (3 + WP) * KS;                        // per warp: [R S' d']^T of the mini-batch (one buffer)
   const int a_elems = 2 * m * SA;                             // per warp: [A_c b]^T of m cameras, two buffers, in JT
   double* sF = sm_dyn + (size_t)warp * f_doubles;
@@ -1362,53 +1366,55 @@ leaf_point_fused_mma_kernel(TreeView t, GroupTable gt, const int* __restrict__ l
   }
   const int p = t.parent[c0];
   if (p < 0) return;      // a root point clique: factored, nothing to extend-add into (block-uniform)
-  // ---- the four warps' sums, added in a fixed order in shared memory (the staging buffers are free now) ----
+  // ---- the four warps' partial sums, in fragment order, to shared memory (the staging buffers are free now) ----
+  const int ntp = NT * (NT + 1) / 2, wstride = 64 * (ntp + m * NAT);   // per warp: tiles of -S'^T S', then the cameras' tiles
   __syncthreads();
-  double* R = sm_dyn;                                          // [WP][WP], upper triangle used (the launch sizes it)
-  for (int round = 0; round < 4; round++) {
-    if (warp == round) {
+  {
+    double* W = sm_dyn + (size_t)warp * wstride + 2 * lane;
 #pragma unroll
-      for (int a = 0; a < NTT; a++)
+    for (int a = 0; a < NTT; a++)
 #pragma unroll
-        for (int b = a; b < NTT; b++)
-          if (b < NT) {
+      for (int b = a; b < NTT; b++)
+        if (b < NT) {
+          double* dst = W + 64 * (a * NT - a * (a - 1) / 2 + (b - a));
+          dst[0] = acc[a][b][0]; dst[1] = acc[a][b][1];
+        }
 #pragma unroll
-            for (int h = 0; h < 2; h++) {
-              double* dst = R + (8 * a + g) * WP + 8 * b + 2 * q + h;
-              *dst = round == 0 ? acc[a][b][h] : *dst + acc[a][b][h];
-            }
-          }
-      __syncwarp();
+    for (int ci = 0; ci < MC; ci++) {
+      if (ci >= m) break;
 #pragma unroll
-      for (int ci = 0; ci < MC; ci++) {
-        if (ci >= m) break;
-#pragma unroll
-        for (int x = 0; x < CT; x++)
-#pragma unroll
-          for (int y = x; y < CT; y++)
-#pragma unroll
-            for (int h = 0; h < 2; h++) {
-              const int lx = 8 * x + g, ly = 8 * y + 2 * q + h;          // entry of [A_c b]^T [A_c b]; column DC = b
-              if (lx <= ly && ly <= DC) {
-                const int i = lx < DC ? ci * DC + lx : s, j = ly < DC ? ci * DC + ly : s;
-                R[i * WP + j] += accA[ci][x * CT - x * (x - 1) / 2 + (y - x)][h];
-              }
-            }
-        __syncwarp();          // (the b^T b of every camera lands on the same entry)
+      for (int x = 0; x < NAT; x++) {
+        double* dst = W + 64 * (ntp + ci * NAT + x);
+        dst[0] = accA[ci][x][0]; dst[1] = accA[ci][x][1];
       }
     }
-    __syncthreads();
   }
-  // one extend-add per run (HessianFactor::updateHessian of the leaf's separator factor)
+  __syncthreads();
+  // ---- one extend-add per run and upper-triangle entry (HessianFactor::updateHessian of the leaf's separator factor) ----
+  // Every entry adds warp 0's -S'^T S', then warp 0's camera terms in camera order, then warp 1's, ...: the order of the
+  // rounds that used to add the warps one after another, so a run's contribution is bitwise what it was.
   double* P = t.arena + t.off[p];
   const int pn = t.nf[p] + t.ns[p] + 1;
-  const int* map = t.ea_map + t.ea_ptr[c0];
-  for (int e = tid; e < w * w; e += 128) {
-    const int i = e / w, j = e - i * w;
-    if (i > j) continue;
-    const int a = map[i], bq = map[j];
+  for (int e = tid; e < w * (w + 1) / 2; e += 128) {
+    int i, j;
+    tri_decode(e, i, j);
+    const int si = (i >> 3) * NT - (i >> 3) * ((i >> 3) - 1) / 2 + ((j >> 3) - (i >> 3));
+    const int so = 64 * si + 8 * (i & 7) + (j & 7);                  // fragment order: lane 4 g + q holds columns 2 q, 2 q + 1
+    // the camera block holding (i, j): i and j in the same camera, or j the rhs column; (s, s) collects every camera's b^T b
+    int cf = -1, cl = -1, lx = 0, ly = 0;
+    if (i < s && (j == s || i / DC == j / DC)) { cf = cl = i / DC; lx = i - cf * DC; ly = j == s ? DC : j - cf * DC; }
+    else if (i == s) { cf = 0; cl = m - 1; lx = ly = DC; }
+    const int ao = 64 * (ntp + (lx >> 3) * CT - (lx >> 3) * ((lx >> 3) - 1) / 2 + ((ly >> 3) - (lx >> 3))) + 8 * (lx & 7) + (ly & 7);
+    double v = 0.0;
+#pragma unroll
+    for (int wp = 0; wp < 4; wp++) {
+      const double* W = sm_dyn + (size_t)wp * wstride;
+      v = wp == 0 ? W[so] : v + W[so];
+      for (int ci = cf; ci <= cl && cf >= 0; ci++) v += W[ao + 64 * NAT * ci];
+    }
+    const int a = sMap[i], bq = sMap[j];
     const int lo = a < bq ? a : bq, hi = a < bq ? bq : a;
-    atomicAdd(P + lo + (size_t)hi * pn, R[i * WP + j]);
+    atomicAdd(P + lo + (size_t)hi * pn, v);
   }
 }
 
