@@ -336,6 +336,31 @@ def leafshapes(model):
         dev.close()
 
 
+def frontshapes(_):
+    """The reduced build of tests/test_front_shapes.py (fronts of at most 65 pivots, small leaves under every dataflow front,
+    a chain of three dataflow fronts) through both builds of the tile dataflow (front_df_kernel<2> / <3>), amalgamation on
+    and off, at every damping: elim_small_kernel, front_df_kernel, backsub_small_kernel and backsub_large_kernel against
+    that file's extended-precision backward-error checks.  The emulator runs a block's threads one at a time between
+    barriers and every CTA in turn, so it checks indexing and arithmetic only: it cannot see a missing fence, a flag
+    published before its data, or any other memory-ordering bug."""
+    import test_front_shapes as T
+    lp = T.front_tree("reduced")
+    for minb in (2, 3):
+        for amalgamate in (True, False):
+            with T.env(B200_DF_MINB=str(minb), B200_NO_AMALGAMATE=None if amalgamate else "1"):
+                dev = capi.LinearDeviceProblem(ctx, lp)
+            sn = dev.supernodes()
+            large = T.backsub_large(T.supernode_table(sn, lp.var_dims))
+            for lam, diag in T.DAMPING:
+                st, e0, e1, _ = dev.solve(lam, diag)
+                assert st == 0
+                rd = T.readout(dev, lp)
+                r, _ = T.check(lp, rd, lam, diag, sn, large)
+                assert max(r.values()) <= 1.0, (minb, amalgamate, lam, diag, r)
+                assert abs(e1 - T.linear_error(lp, rd)) <= 1e-9 * e0
+            dev.close()
+
+
 def coverage(_):
     """Kernel instantiations no fixture reaches (tests/emu/kernel_coverage.py): PriorFactor<Point3> outside the fused
     leaves (points ordered LAST, so their cliques are interior), Dogleg with FP32 Jacobian storage on every factor family
@@ -521,7 +546,7 @@ def allocfail(_):
     dev.close()
 
 
-SCEN = dict(allocfail=allocfail, coverage=coverage, leafshapes=leafshapes, midsize=midsize, edge=edge, bigfront=bigfront, gnc=gnc_scenario, typed=typed, fp32=fp32, linear=linear, marginals=marginals, dogleg=dogleg, gn=gn, mirror=linear_mirror)
+SCEN = dict(allocfail=allocfail, coverage=coverage, leafshapes=leafshapes, frontshapes=frontshapes, midsize=midsize, edge=edge, bigfront=bigfront, gnc=gnc_scenario, typed=typed, fp32=fp32, linear=linear, marginals=marginals, dogleg=dogleg, gn=gn, mirror=linear_mirror)
 for arg in sys.argv[2:]:
     kind, case = arg.split(":")
     t = time.time()

@@ -46,6 +46,8 @@ GROUPS = [
     ["edge:x", "coverage:x", "midsize:cal3_s2", "midsize:bundler", "midsize:bundler@8", "midsize:cal3_s2@8", "midsize:bundler@4", "midsize:cal3_s2@5", "midsize:bundler@3", "bigfront:x"],
     # the BAL point leaves at mixed separator widths and run lengths (tests/test_point_leaf_shapes.py)
     ["leafshapes:cal3_s2", "leafshapes:bundler"],
+    # the dense fronts and their back-substitution at every tile and block boundary (tests/test_front_shapes.py)
+    ["frontshapes:x"],
     # every allocation of problem creation, Dogleg, joint marginals and the Jacobian storage switch failing in turn: nothing leaks
     ["allocfail:x"],
     # the GaussianFactorGraph level, Dogleg, Gauss-Newton
