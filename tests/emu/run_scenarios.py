@@ -361,6 +361,44 @@ def frontshapes(_):
             dev.close()
 
 
+def marginalshapes(_):
+    """The reduced build of tests/test_marginal_shapes.py without amalgamation (a front of 257 pivots with a separator of
+    257 under a 260-pivot root, a chain of three fronts, a second root) through marginal_path_kernel and
+    marginal_joint_kernel: a sample of single-variable marginals (the first and last pivots of both wide fronts, pivot
+    256 of the 257-pivot front, the chain's leaf, the second root) and the joint sets of that file, against its
+    extended-precision forward-error bound; joint diagonal blocks equal to the single marginals bit for bit, cross-tree
+    blocks exactly zero.  Indexing and arithmetic only (see frontshapes)."""
+    import test_front_shapes as FS
+    import test_marginal_shapes as T
+    lp = T.mbuild("reduced")
+    V = T.var_of_node("reduced")
+    with FS.env(B200_NO_AMALGAMATE="1"):
+        dev = capi.LinearDeviceProblem(ctx, lp)
+    qv = [V["A", 0], V["A", 28], V["R", 0], V["R", 27], V["R", 30], V["k0", 0], V["Q", 2]]
+    singles = {v: dev.marginal_covariance(v) for v in qv}
+    rd = FS.readout(dev, lp)
+    sets = T.joint_sets("reduced")
+    joints = [(vs, dev.joint_marginal_covariance(vs)) for vs in sets]
+    sn = dev.supernodes()
+    t = FS.supernode_table(sn, lp.var_dims)
+    assert {257} <= set(t["f"].tolist()) and 257 in set(t["s"].tolist())
+    r, _ = FS.check(lp, rd, 0.0, False, sn, FS.backsub_large(t))
+    assert max(r.values()) <= 1.0, r
+    rs, rj = T.check_marginals(lp, rd, singles, joints)
+    assert rs <= 1.0 and rj <= 1.0, (rs, rj)
+    dof = lp.dof_offsets()
+    for vs, S in joints:
+        o = np.concatenate([[0], np.cumsum(lp.var_dims[list(vs)])])
+        for a, u in enumerate(vs):
+            if u in singles:
+                assert np.array_equal(S[o[a]:o[a + 1], o[a]:o[a + 1]], singles[u]), (vs, u)
+        if V["Q", 0] in vs or V["Q", 1] in vs:
+            q = [a for a, u in enumerate(vs) if u in (V["Q", 0], V["Q", 1])][0]
+            rest = np.concatenate([np.arange(o[a], o[a + 1]) for a in range(len(vs)) if a != q])
+            assert np.all(S[np.ix_(rest, np.arange(o[q], o[q + 1]))] == 0.0), vs
+    dev.close()
+
+
 def coverage(_):
     """Kernel instantiations no fixture reaches (tests/emu/kernel_coverage.py): PriorFactor<Point3> outside the fused
     leaves (points ordered LAST, so their cliques are interior), Dogleg with FP32 Jacobian storage on every factor family
@@ -546,7 +584,7 @@ def allocfail(_):
     dev.close()
 
 
-SCEN = dict(allocfail=allocfail, coverage=coverage, leafshapes=leafshapes, frontshapes=frontshapes, midsize=midsize, edge=edge, bigfront=bigfront, gnc=gnc_scenario, typed=typed, fp32=fp32, linear=linear, marginals=marginals, dogleg=dogleg, gn=gn, mirror=linear_mirror)
+SCEN = dict(allocfail=allocfail, coverage=coverage, leafshapes=leafshapes, frontshapes=frontshapes, marginalshapes=marginalshapes, midsize=midsize, edge=edge, bigfront=bigfront, gnc=gnc_scenario, typed=typed, fp32=fp32, linear=linear, marginals=marginals, dogleg=dogleg, gn=gn, mirror=linear_mirror)
 for arg in sys.argv[2:]:
     kind, case = arg.split(":")
     t = time.time()

@@ -59,6 +59,7 @@ SMALL_MAX_N = 48          # kSmallMaxN (kernels.cuh): fronts up to this size are
 THIN_F = 8                # plan_levels (engine.cu): dataflow fronts of at most 8 pivots are back-substituted one warp each
 BLOCK = 32                # kDfB (front_df.cuh): the pivot blocks, and the diagonal blocks W = R_bb^-1 is kept for
 LEAF_MAX_F = 6            # kLeafMaxF (kernels.cuh): typed problems' leaves up to this many pivots take the fused leaf kernels
+JACOBIAN_MAX_ARITY = 8    # B200_JACOBIAN_MAX_ARITY (include/gtsam_b200.h)
 F_GRID = (1, 2, 8, 9, 31, 32, 33, 63, 64, 65, 127, 128, 129, 160, 161)
 S1_GRID = (1, 31, 32, 33, 64, 65, 129)
 DAMPING = ((0.0, False), (1e-3, False), (1e-2, True))
@@ -102,9 +103,11 @@ def build_nodes(name):
 BUILDS = ("level0", "nested", "graded")
 
 
-def front_tree(name, seed=5):
-    """The LinearProblem of build `name` (module docstring); elimination order = node order."""
-    nodes = build_nodes(name)
+def front_tree(name, seed=5, nodes=None, graded=None):
+    """The LinearProblem of build `name` (module docstring), or of the node list `nodes` (as build_nodes returns) under that
+    name; elimination order = node order.  graded: scale the columns as build "graded" does (default: name == "graded")."""
+    nodes = build_nodes(name) if nodes is None else nodes
+    graded = name == "graded" if graded is None else graded
     rng = np.random.default_rng(seed)
     var, dims = {}, []
     for node, vd, _ in nodes:
@@ -113,7 +116,7 @@ def front_tree(name, seed=5):
             dims.append(d)
     dof = np.concatenate([[0], np.cumsum(dims)])
     scale = np.ones(dof[-1])
-    if name == "graded":
+    if graded:
         scale = 10.0 ** rng.uniform(-4, 4, size=dof[-1])
         # the last two pivots of every front stay unscaled: a ratio of 2^12 between them, or a single pivot below 2^-12,
         # is the underconstrained-system test (gtsam's Cholesky), which would report the system as indeterminate
@@ -131,11 +134,16 @@ def front_tree(name, seed=5):
 
     for node, vd, sep in nodes:
         keys = [var[(node, k)] for k in range(len(vd))] + [var[r] for r in sep]
-        kd, Ab = jacobian(keys, 3)
-        if name == "nested" and node == "M2":
-            hgroups.append(LN.HessianGroup(kd, np.array([keys]), (Ab.T @ Ab)[None]))
-        else:
-            groups.append(LN.JacobianGroup(Ab.shape[0], kd, np.array([keys]), Ab.T[None]))
+        # a node of more than JACOBIAN_MAX_ARITY keys: factors on its first variable and up to 7 more each; eliminating
+        # that variable first joins them all into one clique, as one dense factor would
+        parts = [keys] if len(keys) <= JACOBIAN_MAX_ARITY else \
+            [[keys[0]] + keys[i:i + JACOBIAN_MAX_ARITY - 1] for i in range(1, len(keys), JACOBIAN_MAX_ARITY - 1)]
+        for part in parts:
+            kd, Ab = jacobian(part, 3)
+            if name == "nested" and node == "M2":
+                hgroups.append(LN.HessianGroup(kd, np.array([part]), (Ab.T @ Ab)[None]))
+            else:
+                groups.append(LN.JacobianGroup(Ab.shape[0], kd, np.array([part]), Ab.T[None]))
         if not sep:
             for k in keys:
                 kd, Ab = jacobian([k], 2)

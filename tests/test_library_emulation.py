@@ -48,6 +48,8 @@ GROUPS = [
     ["leafshapes:cal3_s2", "leafshapes:bundler"],
     # the dense fronts and their back-substitution at every tile and block boundary (tests/test_front_shapes.py)
     ["frontshapes:x"],
+    # the marginal kernels on a front wider than one CTA, a chain and a forest (tests/test_marginal_shapes.py)
+    ["marginalshapes:x"],
     # every allocation of problem creation, Dogleg, joint marginals and the Jacobian storage switch failing in turn: nothing leaks
     ["allocfail:x"],
     # the GaussianFactorGraph level, Dogleg, Gauss-Newton
